@@ -68,11 +68,12 @@ def prefill_flops(m, n):
 
 
 def measured_peaks():
+    # fallback: NVIDIA's H100 SXM data sheet (3.35 TB/s HBM3, 989 TFLOP/s dense bf16 at up to 700 W), not a measurement
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops", 1590.0), d.get("bf16_tflops_sustained", 1400.0), "measured"
-    return 6650.0, 1590.0, 1400.0, "fallback"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops", 989.0), d.get("bf16_tflops_sustained", 989.0), "measured"
+    return 3350.0, 989.0, 989.0, "H100 SXM data sheet"
 
 
 def pct(xs, q):
@@ -83,7 +84,7 @@ def pct(xs, q):
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons during the timed region (recipe: B200_PROFILING.md)."""
+    """nvidia-smi clocks + throttle reasons during the timed region (read-only queries)."""
 
     def __init__(self, index=0):
         self.rows, self.proc, self.index = [], None, index
@@ -221,7 +222,7 @@ def workload_config(args, model, tp):
             if args.model == "8b" else "tiny-geometry debug run (NOT the benchmark config)",
             "model_geometry": model, "prompt_tokens": PROMPT, "generated_tokens": GEN, "batch": args.batch,
             "parallelism": "tp%d" % tp, "weights": "synthetic seed 0, N(0,0.02^2) via integer hash",
-            "l2": "inputs larger than L2: 15 GB of weights are streamed per decode step (126 MB L2)"}
+            "l2": "inputs larger than L2: 15 GB of weights are streamed per decode step (50 MB L2 on H100)"}
 
 
 # ------------------------------------------------------------------------------ GPU arm -----
@@ -255,11 +256,9 @@ def gemv_microbench(model, hbm_peak):
     torch.cuda.synchronize()
     us = a.elapsed_time(b) * 1e3 / iters
     bytes_ = n_out * H * 2
-    traffic = 244.44e6 if (n_out, H) == (28672, 4096) else None
     return {"kernel": "gemv_ks_kernel<1,SILU_MUL,NORM,1> %dx%d (gate/up, fused RMSNorm + SiLU*up)" % (n_out, H),
             "bytes_per_launch": bytes_, "us_per_launch": us, "achieved": bytes_ / us / 1e3, "unit": "GB/s",
-            "frac": bytes_ / us / 1e3 / hbm_peak, "traffic": traffic,
-            "traffic_source": "not measured in this run: dram__bytes_read.sum + dram__bytes_write.sum of one launch in the committed ncu --set full capture profiles/r1_final_gemv_ks_ncu_full.txt (241.20 + 3.24 MB)"}
+            "frac": bytes_ / us / 1e3 / hbm_peak}
 
 
 def run_ours(args):
@@ -366,8 +365,10 @@ def run_ours(args):
         sampler.start()
     t0 = time.perf_counter()
     first_to_last_ms, n_dec_tokens, req_tps, req_ms = 0.0, 0, [], []
+    last_tokens = None
     for i in range(args.steps):
         toks, _ = run_requests([make_prompt(i * args.batch + j, model["vocab"]) for j in range(args.batch)], GEN)
+        last_tokens = toks
         lo, hi = [], []
         for tk in toks:
             assert len(tk) == GEN, "request produced %d tokens" % len(tk)
@@ -386,6 +387,15 @@ def run_ours(args):
     if world > 1:
         dist.all_reduce(vals, op=dist.ReduceOp.MAX)
     gpu_ms_dec, gpu_ms_pre, wall_ms, ftl_ms, req_ms_sum = [float(v) for v in vals]
+    if args.dump_outputs and rank == 0 and last_tokens is not None:
+        # what a caller of the timed path receives in its last step: the generated token ids of every request
+        # ([batch, GEN], exact integers in float64) and the prompts they answer; prompts are seeded by step index
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "tokens.npy"),
+                np.array([[t["token_id"] for t in tk] for tk in last_tokens], dtype=np.float64))
+        i = args.steps - 1
+        np.save(os.path.join(args.dump_outputs, "prompts.npy"),
+                np.array([make_prompt(i * args.batch + j, model["vocab"]) for j in range(args.batch)], dtype=np.float64))
     dec_tokens, pre_tokens, dec_steps = d("tokens_decode"), d("tokens_prefill"), d("steps_decode")
     main_launches = d("kernel_launches")
     decode_tok_s = dec_tokens / (gpu_ms_dec / 1e3)
@@ -471,8 +481,6 @@ def run_ours(args):
                         "roofline": {"bound": "tensor", "achieved": pre_tf, "peak": tf_burst, "unit": "TFLOP/s",
                                      "frac": pre_tf / tf_burst, "peak_source": peak_src + " (burst cuBLAS bf16)"}},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": hbm_peak, "unit": "GB/s", "frac": achieved / hbm_peak,
-                         "traffic": (32 * (50.39e6 + 33.60e6 + 244.44e6 + 120.83e6) + 1050.7e6) if (args.model == "8b" and tp == 1 and args.batch == 1) else None,
-                         "traffic_source": "not measured in this run: sum over the step's projections of dram__bytes_read+write from the committed ncu --set full captures under profiles/ (lm_head: algorithmic)",
                          "peak_source": peak_src,
                          "what": "whole decode step (%.2f GB algorithmic per step per GPU / %.3f ms CUDA-event step time)" % (bytes_step / 1e9, step_s * 1e3),
                          "kernel": kern},
@@ -539,6 +547,8 @@ def main():
     ap.add_argument("--cpu-prompt", type=int, default=32)
     ap.add_argument("--cpu-gen", type=int, default=8)
     ap.add_argument("--cpu-q4-child", action="store_true", help=argparse.SUPPRESS)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's outputs (tokens.npy, prompts.npy) to DIR")
     args = ap.parse_args()
     if args.cpu_q4_child:     # the Q4_0 x Q8_0 leg of the CPU baseline, run by run_ours in its own process
         from llmlb_b200.ffi import LLAMA3_8B, LLAMA_TINY

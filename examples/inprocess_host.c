@@ -14,7 +14,7 @@
  *   end of stream: usage, lease, TPS (proxy.rs:147-203, 290-368)
  *                                                     llmlb_acc_finalize, llmlb_lm_lease_complete, llmlb_lm_update_tps
  *
- * Build (real engine; needs a B200):
+ * Build (real engine; needs an H100):
  *   gcc -std=c99 -O2 -Iinclude examples/inprocess_host.c -Lllmlb_b200 -lllmlb_b200 -lllmlb_host -Wl,-rpath,$PWD/llmlb_b200 -o inprocess_host
  * The CPU suite builds it against tests/support/fake_engine.cpp (same ABI, scripted tokens): tests/test_inprocess_host_cpu.py.
  *

@@ -1,4 +1,4 @@
-// Locates libllmlb_b200.so (built by `python -m llmlb_b200.build`, nvcc sm_100a) and tells rustc to
+// Locates libllmlb_b200.so (built by `python -m llmlb_b200.build`, nvcc sm_90a) and tells rustc to
 // link it.  LLMLB_B200_LIB_DIR overrides the default (../../llmlb_b200 relative to this crate).
 use std::env;
 use std::path::PathBuf;

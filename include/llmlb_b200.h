@@ -1,5 +1,5 @@
 /*
- * llmlb_b200.h — C ABI of the B200-native in-process inference backend for llmlb.
+ * llmlb_b200.h — C ABI of the H100-native in-process inference backend for llmlb.
  *
  * This is the drop-in boundary (SURVEY.md §8b).  In the reference, model work is
  * reached through one HTTP call: `reqwest POST {base_url}/v1/...` at
@@ -75,14 +75,14 @@ typedef struct llmlb_engine_config {
   uint64_t synthetic_seed;   /* weights are generated on-device from this seed (see
                                 llmlb_engine_load_tensor to overwrite with real ones) */
   uint32_t use_cuda_graphs;  /* capture decode steps per batch width */
-  uint32_t gemm_impl;        /* 0 = tcgen05/TMEM/TMA tiles (default), 1 = mma.sync tiles */
+  uint32_t gemm_impl;        /* 0 = wgmma/TMA tiles (default), 1 = mma.sync tiles */
   uint32_t lookahead;        /* decode steps in flight before the host reads tokens (0 = 2) */
   /* Back-pressure, mirroring the gateway's own queue (llmlb/src/config.rs:80-99, QueueConfig) and its
    * per-request inference timeout (llmlb/src/types/endpoint.rs:389).  0 = no limit. */
   uint32_t queue_max;          /* waiting requests beyond this: submit returns LLMLB_E_QUEUE_FULL (gateway: 429) */
   uint32_t queue_timeout_ms;   /* a request still waiting for admission after this finishes QUEUE_TIMEOUT (504) */
   uint32_t request_timeout_ms; /* a request not finished this long after submit finishes DEADLINE (504 timeout) */
-  uint32_t attn_impl;          /* prefill attention: 0 = tcgen05 + TMEM + TMA (default), 1 = mma.sync baseline */
+  uint32_t attn_impl;          /* prefill attention: 0 = wgmma + TMA (default), 1 = mma.sync baseline */
   uint32_t tp_proto;           /* tensor-parallel decode exchange: bit 0: 0 = {value, epoch} pairs (default), 1 = values + flags;
                                   bit 1: 1 = owner CTAs fold the partials and the consumer grid gathers the result through L2 */
   uint32_t reserved[3];
@@ -224,7 +224,7 @@ enum { LLMLB_EPI_STORE_BF16 = 0,   /* out_bf16[t,n]  = acc                      
 int llmlb_op_gemv(const void* w_bf16, const void* x, const void* gain_bf16, float eps, void* out,
                   uint32_t n_tokens, uint32_t n_out, uint32_t k, uint32_t epilogue,
                   uint32_t out_stride, void* stream);
-/* prefill / batched path: out[t,n] = sum_k x[t,k]*W[n,k] on tensor cores (tcgen05 + TMEM + TMA tiles).
+/* prefill / batched path: out[t,n] = sum_k x[t,k]*W[n,k] on tensor cores (wgmma + TMA tiles).
  * impl must be 0: the round-1 mma.sync (1) and stream-K (2) variants left the library (tools/experiments/) and return
  * LLMLB_E_UNSUPPORTED.  x is bf16 [n_tokens,k]; k a multiple of 8; SILU_MUL needs an even n_out (interleaved gate/up rows). */
 int llmlb_op_gemm(const void* w_bf16, const void* x_bf16, void* out, uint32_t n_tokens,
@@ -245,7 +245,7 @@ int llmlb_op_prefill_attention(const void* qkv_bf16, const void* k_pages, const 
                                const int32_t* block_tables, uint32_t bt_stride,
                                const int32_t* tiles, uint32_t n_tiles, void* out_bf16,
                                uint32_t n_heads, uint32_t n_kv_heads, void* stream);
-/* a2.6 on the 5th-generation tensor cores (tcgen05.mma, S and PV in TMEM, Q/K/V staged by TMA; V is
+/* a2.6 on the Hopper tensor cores (wgmma, S and O in registers, Q/K/V staged by TMA; V is
  * consumed MN-major straight from its [token][d] pages).  Same contract as above with q tiles of up to
  * 128 rows; k_pages / v_pages are ONE layer's pool [n_pages][n_kv][64][128]; n_tokens = rows of qkv. */
 int llmlb_op_prefill_attention_tc(const void* qkv_bf16, uint32_t n_tokens, const void* k_pages,

@@ -1,4 +1,4 @@
-"""Builds libllmlb_b200.so (CUDA kernels + engine + C ABI) in-tree with nvcc for sm_100a.
+"""Builds libllmlb_b200.so (CUDA kernels + engine + C ABI) in-tree with nvcc for sm_90a (H100).
 
 No torch involvement: the library links only against the CUDA runtime.  The .so lands next to
 this file so that it travels with the repo snapshot to the GPU box.
@@ -16,13 +16,14 @@ LIB = os.path.join(HERE, "libllmlb_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 SOURCES = ["elementwise.cu", "gemv.cu", "gemv_ks.cu", "gemm_tc.cu", "gemm_tc2.cu", "attention.cu", "attention_tc.cu",
            "sampling.cu", "tp_exchange.cu", "engine.cu"]
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
 
 def _digest(path):
     h = hashlib.sha256()
     for dep in [path, os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "tc_common.cuh"), os.path.join(CSRC, "tp_common.cuh"),
+                os.path.join(CSRC, "wgmma.cuh"),
                 os.path.join(HERE, "..", "include", "llmlb_b200.h"), __file__]:
         with open(dep, "rb") as f:
             h.update(f.read())
@@ -57,7 +58,7 @@ def build(verbose=False, force=False):
     objs = [o for o, _, _ in results]
     changed = any(c for _, c, _ in results)
     if changed or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a",
+        cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a",
                "-lcudart", "-lpthread"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:

@@ -685,8 +685,7 @@ namespace llmlb {
 constexpr int kDamThreads = 32;
 // K/V move through a 3-stage ring of 32-token half pages: 48 KiB + q per CTA, so FOUR one-warp CTAs
 // share an SM and the 512 CTAs of a 64-stream step are resident at once (with whole pages and
-// two stages only three fit: a second, mostly empty wave doubled the kernel's time — ncu,
-// profiles/r1_decode_attn_mma_ncu_full.txt)
+// two stages only three fit: a second, mostly empty wave doubled the kernel's time)
 constexpr int kDamChunk = 32;
 constexpr int kDamStages = 3;
 constexpr int kDamSmem = kDamStages * 2 * kDamChunk * kHeadDim * 2 + kDecHeads * kHeadDim * 2;

@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels of llmlb_b200.
+// Shared helpers for the sm_90a kernels of llmlb_b200.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -15,7 +15,7 @@ extern unsigned int g_dbg_no_pdl;   // bit mask: 1 plain GEMV, 2 tp consumer GEM
 
 constexpr int kHeadDim = 128;        // Llama-3 head width (the only one the kernels accept)
 constexpr int kPageTokens = 64;      // tokens per KV page
-constexpr int kNumSMs = 148;         // B200
+constexpr int kNumSMs = 132;         // H100 SXM
 
 // thread-local error text behind llmlb_last_error()
 void set_error(const std::string& s);

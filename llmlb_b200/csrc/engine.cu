@@ -66,7 +66,7 @@ int gemv_tp_push(const TpCtx& ctx, uint32_t coll_out, const void* w, const void*
 int ar_allreduce_add(const TpCtx& P, uint64_t off, float* x, uint64_t n, cudaStream_t st);
 int ar_allgather_cols(const TpCtx& P, uint64_t off, float* out, uint32_t rows, uint32_t cols_local, cudaStream_t st);
 constexpr uint32_t kTpMaxSplit = 4;   // K-split parts a push-RS GEMM may use (slot capacity)
-// prefill attention on tcgen05 (attention_tc.cu)
+// prefill attention on wgmma (attention_tc.cu)
 int make_tmap_attn_q(CUtensorMap* m, const void* qkv, uint64_t n_tokens, uint64_t width);
 int make_tmap_attn_kv(CUtensorMap* m, const void* pool, uint64_t n_layers, uint64_t n_pages, uint64_t n_kv);
 int prefill_attention_tc_launch(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, uint32_t layer,
@@ -364,7 +364,7 @@ struct llmlb_engine {
   float* x_last = nullptr;       // [max_seqs][hidden]
   void* attn_ws = nullptr;
   CUtensorMap m_y[5]{}, m_attn[5]{}, m_h[5]{};  // box rows 16,32,64,128,256
-  CUtensorMap m_attn_q{}, m_kpool{}, m_vpool{};  // tcgen05 prefill attention: q rows of qkv, the K / V pools (5-D)
+  CUtensorMap m_attn_q{}, m_kpool{}, m_vpool{};  // wgmma prefill attention: q rows of qkv, the K / V pools (5-D)
   uint32_t pf_tile = 128;                         // q rows per prefill-attention tile (64 for the mma.sync baseline)
 
   // per-step metadata (device) + pinned staging ring
@@ -522,9 +522,9 @@ int llmlb_engine::init() {
     set_error("kv_block_tokens must be 64"); return LLMLB_E_INVALID_ARG;
   }
   if (!(tp == 1 || tp == 2 || tp == 4 || tp == 8) || rank >= tp) { set_error("bad tp_size/tp_rank"); return LLMLB_E_INVALID_ARG; }
-  if (cfg.gemm_impl != 0) { set_error("gemm_impl: only 0 (tcgen05 tiles) is built into the library"); return LLMLB_E_INVALID_ARG; }
+  if (cfg.gemm_impl != 0) { set_error("gemm_impl: only 0 (wgmma tiles) is built into the library"); return LLMLB_E_INVALID_ARG; }
   if (cfg.tp_proto > 3) { set_error("tp_proto: bit 0 = flags instead of value+epoch pairs, bit 1 = owner-fold + gather consumer"); return LLMLB_E_INVALID_ARG; }
-  if (cfg.attn_impl > 1) { set_error("attn_impl: 0 (tcgen05) or 1 (mma.sync baseline)"); return LLMLB_E_INVALID_ARG; }
+  if (cfg.attn_impl > 1) { set_error("attn_impl: 0 (wgmma) or 1 (mma.sync baseline)"); return LLMLB_E_INVALID_ARG; }
   if (M.n_kv_heads == 0 || M.n_heads % M.n_kv_heads || M.n_kv_heads % tp || M.ffn % tp || M.vocab % tp ||
       ((M.n_heads / M.n_kv_heads) % 4) || M.hidden % 8 || (M.ffn / tp) % 8 || (M.vocab / tp) % 4 ||
       M.n_layers == 0 || M.vocab == 0) {
@@ -753,9 +753,9 @@ int llmlb_engine::proj(const CUtensorMap& mw, const void*, const void*, const CU
   if (wait_coll >= 0 && !dbg_no_agwait) {   // tensor parallel: the activation operand is y of that collective (its all-gather flags gate the loads)
     tpp.ctx = tpc; tpp.wait_coll_plus1 = uint32_t(wait_coll) + 1;
   }
-  // A projection whose CTA-pair tiles fill whole waves plus a short ragged one (gate/up at 512 tokens: 224 tiles on
-  // 74 pairs = 3.03 waves, run as 4): the rows of the ragged wave go to a second launch of 128-row tiles with the
-  // in-kernel K-split (all SMs, a fraction of a tile time) and the pair kernel runs exact waves.
+  // A projection whose CTA-pair tiles fill whole waves plus a short ragged one (at most two 256-row slabs): the rows
+  // of the ragged wave go to a second launch of 128-row tiles with the in-kernel K-split (all SMs, a fraction of a
+  // tile time) and the pair kernel runs exact waves.
   const bool store_epi = epi == LLMLB_EPI_STORE_BF16 || epi == LLMLB_EPI_SILU_MUL || epi == LLMLB_EPI_STORE_F32;
   if (store_epi && T > 128 && n_out % 256 == 0 && tpp.sk_ws && !dbg_no_wave_tail) {
     const uint32_t t_tiles = ceil_div(T, 256u), m_pairs = n_out / 256, pairs = uint32_t(kNumSMs / 2);

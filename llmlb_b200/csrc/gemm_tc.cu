@@ -1,4 +1,4 @@
-// Prefill / batched-decode projections on the 5th-gen tensor cores (SURVEY §8 a2.3/8/9/10/11).
+// Prefill / batched-decode projections on the Hopper tensor cores (wgmma, SURVEY §8 a2.3/8/9/10/11).
 //
 //   out[t, n] = sum_k X[t, k] * W[n, k]        X bf16 [T, K], W bf16 [N, K] (both K-major)
 //
@@ -6,11 +6,9 @@
 // as the N operand (BN = 16..256 picked from T), so one kernel serves 16-token batched decode
 // (HBM-bound: W streamed once through a deep TMA ring) and 512-token prefill (tensor-bound).
 // Warp roles (384 threads, 1 CTA/SM, persistent over tiles):
-//   warp 0 lane 0 : TMA producer   — cp.async.bulk.tensor 2D, 128B-swizzled 64-wide K slabs
-//   warp 1 lane 0 : MMA issuer     — tcgen05.mma.cta_group::1.kind::f16, fp32 accum in TMEM
-//   warp 2        : TMEM allocator — 2 accumulator stages (epilogue of tile i overlaps MMA of i+1)
-//   warps 4..11   : epilogue       — tcgen05.ld 32x32b (two warps per TMEM lane quarter, half the
-//                                    columns each), fused residual-add / SiLU*up / store
+//   warp 0 lane 0   : TMA producer  — cp.async.bulk.tensor 2D, 128B-swizzled 64-wide K slabs
+//   warpgroups 1, 2 : consumers     — wgmma.mma_async m64nBNk16 on 64 weight rows each, fp32 accumulators in
+//                                     registers, then the fused epilogue (residual-add / SiLU*up / store) from them
 // Split-K (residual epilogue only) uses fp32 red.global.add.
 #include <cuda.h>
 
@@ -47,9 +45,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + Cfg::kStages;
-  uint64_t* tfull_bar = bars + 2 * Cfg::kStages;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t k_blocks_total = (K + kBK - 1) / kBK;
@@ -64,27 +59,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < Cfg::kStages; ++i) {
       mbar_init(full_bar + i, 1);
-      mbar_init(empty_bar + i, 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(tfull_bar + i, 1);
-      mbar_init(tempty_bar + i, 8);
+      mbar_init(empty_bar + i, 8);   // one arrival per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(tmem_slot)),
-                 "r"(uint32_t(Cfg::kTmemCols))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // debug timeline: cycles each role spent blocked (producer on free slots, MMA issuer on data,
-  // epilogue on finished accumulators) — see tools/gemm_stalls.py
+  // debug timeline: cycles each role spent blocked (producer on free slots, each consumer warpgroup on data)
+  // — see tools/gemm_stalls.py
   const TraceBuf tb = d_trace_tc;
   __shared__ long long stall[4];
   const long long c_begin = clock64();
@@ -103,10 +84,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
     if (lane == 0) {
       uint32_t stage = 0, phase = 0;
       // L2 prefetch cursor: runs kPrefetchAhead K-slabs ahead of the smem loads (weights only —
-      // the activation operand is small and L2-resident).  The smem ring holds 3 slabs in flight
-      // (~1.5k MMA cycles); an HBM miss costs 3-4k, an L2 hit ~1k.
-      // (a 512-byte-per-row prefetch view through a second, unswizzled map measured slower:
-      // lm_head at 64 tokens 188 -> 203 us)
+      // the activation operand is small and L2-resident)
       constexpr uint32_t kPrefetchAhead = 12;
       uint32_t p_tile = blockIdx.x, p_kb = 0, p_kb1 = 0, p_mt = 0;
       auto p_load = [&]() {
@@ -163,53 +141,21 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
       }
       if (!dep_ready) release_deferred();   // fewer K blocks than stages
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      uint32_t stage = 0, phase = 0, acc = 0, acc_phase = 0;
-      for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        uint32_t mt, tt, ks;
-        decode_tile(tile, mt, tt, ks);
-        const uint32_t kb0 = ks * k_per_split;
-        const uint32_t kb1 = min(k_blocks_total, kb0 + k_per_split);
-        mbar_wait(tempty_bar + acc, acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * BN;
-        for (uint32_t kb = kb0; kb < kb1; ++kb) {
-          { const long long c0 = clock64(); mbar_wait(full_bar + stage, phase); c_wait += clock64() - c0; }
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-          const uint32_t sb = sa + kBM * kBK * 2;
-          const uint64_t adesc = make_sw128_desc(sa);
-          const uint64_t bdesc = make_sw128_desc(sb);
-#pragma unroll
-          for (int k = 0; k < kBK / 16; ++k) {
-            // advance 32 B (16 bf16) inside the 128 B swizzle row: +2 in the 16-byte address field
-            tc_mma(tmem_d, adesc + uint64_t(k * 2), bdesc + uint64_t(k * 2), Cfg::kIdesc,
-                   (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          tc_commit(empty_bar + stage);  // frees the smem slot when these MMAs retire
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-        }
-        tc_commit(tfull_bar + acc);      // accumulator complete -> epilogue
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
   } else if (warp >= 4) {
-    const uint32_t q = warp & 3;  // TMEM lane quarter this warp may read
-    uint32_t acc = 0, acc_phase = 0;
+    const uint32_t wg = (warp >> 2) - 1;      // consumer warpgroup: weight rows [64 wg, 64 wg + 64) of the tile
+    const uint32_t wrow = wg * 64 + (warp & 3) * 16;   // first tile row of this warp's fragment
+    uint32_t stage = 0, phase = 0;
     if (pdl) asm volatile("griddepcontrol.wait;" ::: "memory");   // outputs may alias what earlier kernels read
     uint32_t ep_ll = 0;
     if constexpr (EPI == kEpiPushRSLL) ep_ll = tp_epoch32(tp.ctx, tp.coll);   // the step counter is final after the wait
     for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
       uint32_t mt, tt, ks;
       decode_tile(tile, mt, tt, ks);
-      { const long long c0 = clock64(); mbar_wait(tfull_bar + acc, acc_phase); c_wait += clock64() - c0; }
-      tc_fence_after();
-      const uint32_t n = mt * kBM + q * 32 + lane;      // output feature of this thread
+      const uint32_t kb0 = ks * k_per_split;
+      const uint32_t kb1 = min(k_blocks_total, kb0 + k_per_split);
+      float acc[BN / 2];
+      tc_mainloop<BN, false>(acc, smem, full_bar, empty_bar, kb0, kb1, wg, stage, phase, c_wait);
       const uint32_t t0 = tt * BN;
-      // two warps share a TMEM lane quarter: each takes half of the token columns
-      constexpr uint32_t kColsPerWarp = (BN / 2 >= 16) ? BN / 2 : 16;
-      const uint32_t c_begin = ((warp - 4) >> 2) * kColsPerWarp;
       if constexpr (EPI == LLMLB_EPI_STORE_BF16 || EPI == LLMLB_EPI_SILU_MUL || EPI == LLMLB_EPI_STORE_F32) {
         if (split_k > 1) {
           // ---- in-kernel K-split: the split_k CTAs of an output tile each park their fp32 partial in the
@@ -217,23 +163,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
           // group (sum over the parts in part order: deterministic), so the reduction itself is spread
           // over the CTAs that did the products.  All CTAs of the grid are co-resident (one tile per CTA,
           // grid <= SM count) and nobody waits before it has parked its own part.
+          // Workspace tile layout: [16-token group][128 rows][16 tokens].
           const uint32_t otile = (mt - m_tile0) * t_tiles + tt;
           float* wtile = tp.sk_ws + size_t(otile) * split_k * (BN * kBM);
           float* wmine = wtile + size_t(ks) * (BN * kBM);
-#pragma unroll 1
-          for (uint32_t c = c_begin; c < c_begin + kColsPerWarp && c < BN; c += 16) {
-            if (t0 + c >= n_tokens) break;
-            uint32_t r[16];
-            tc_ld16(tmem_base + ((q * 32) << 16) + acc * BN + c, r);
-            tc_wait_ld();
-            float4* dst = reinterpret_cast<float4*>(wmine + (c >> 4) * (16 * kBM) + (q * 32 + lane) * 16);
 #pragma unroll
-            for (int j = 0; j < 4; ++j)
-              dst[j] = make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]), __uint_as_float(r[4 * j + 2]), __uint_as_float(r[4 * j + 3]));
+          for (int c = 0; c < BN / 8; ++c) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              const uint32_t row = wrow + (lane >> 2) + 8 * i, col = 8 * c + 2 * (lane & 3);
+              *reinterpret_cast<float2*>(wmine + (col >> 4) * (16 * kBM) + row * 16 + (col & 15)) =
+                  make_float2(acc[4 * c + 2 * i], acc[4 * c + 2 * i + 1]);
+            }
           }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(tempty_bar + acc);
           epi_bar();
           if (threadIdx.x == 128) {
             __threadfence();                        // the CTA's parked part is performed device-wide before its arrival
@@ -294,87 +236,18 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
           }
           // second pass over the counter: the CTA that sees every part gone through the meeting point zeroes it
           if (threadIdx.x == 128 && atomicAdd(tp.sk_cnt + otile, 1u) == 2 * split_k - 1) atomicExch(tp.sk_cnt + otile, 0u);
-          if (++acc == 2) { acc = 0; acc_phase ^= 1; }
           continue;
         }
       }
-#pragma unroll 1
-      for (uint32_t c = c_begin; c < c_begin + kColsPerWarp && c < BN; c += 16) {
-        if (t0 + c >= n_tokens) break;                  // warp-uniform
-        uint32_t r[16];
-        tc_ld16(tmem_base + ((q * 32) << 16) + acc * BN + c, r);
-        tc_wait_ld();
-        if constexpr (EPI == kEpiPushRSLL) {
-          // lanes (2i, 2i+1) hold output features (n, n+1) of the same tokens: one 8-byte word {bf16 n, bf16 n+1, epoch}
-          // per token; even lanes send the even token columns, odd lanes the odd ones
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const float v = __uint_as_float(r[j]);
-            const float other = __shfl_xor_sync(0xffffffffu, v, 1);
-            const uint32_t t = t0 + c + j;
-            if (((j ^ lane) & 1) == 0 && (n | 1) < n_out && t < n_tokens) {
-              const float lo = (lane & 1) ? other : v, hi = (lane & 1) ? v : other;
-              const uint32_t owner = t / tp.rpr, tl = t - owner * tp.rpr;
-              uint2 w;
-              w.x = pack_bf16(lo, hi);
-              w.y = ep_ll;
-              st_peer_u2(reinterpret_cast<uint2*>(s_peer_slot[owner]) +
-                             (size_t(tp.ctx.rank * split_k + ks) * tp.rpr + tl) * (out_stride / 2) + (n >> 1), w);
-            }
-          }
-        } else if constexpr (EPI == LLMLB_EPI_SILU_MUL) {
-          __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(out);
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const float v = __uint_as_float(r[j]);
-            const float other = __shfl_xor_sync(0xffffffffu, v, 1);
-            // lanes (2i, 2i+1) hold (gate_i, up_i); even lanes finish even columns, odd lanes odd ones
-            if (((j ^ lane) & 1) == 0 && (n | 1) < n_out && t0 + c + j < n_tokens) {
-              const float g = (lane & 1) ? other : v, u = (lane & 1) ? v : other;
-              const float s = __fdividef(g, 1.f + __expf(-g));  // IEEE division was ~half of the epilogue's instructions
-              o[size_t(t0 + c + j) * out_stride + (n >> 1)] = __float2bfloat16_rn(s * u);
-            }
-          }
-        } else {
-          if (n < n_out) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const uint32_t t = t0 + c + j;
-              if (t < n_tokens) {
-                const float v = __uint_as_float(r[j]);
-                const size_t idx = size_t(t) * out_stride + n;
-                if constexpr (EPI == LLMLB_EPI_STORE_BF16)
-                  reinterpret_cast<__nv_bfloat16*>(out)[idx] = __float2bfloat16_rn(v);
-                else if constexpr (EPI == LLMLB_EPI_STORE_F32)
-                  reinterpret_cast<float*>(out)[idx] = v;
-                else if constexpr (EPI == kEpiPartialF32)  // deterministic split-K: slot ks of the workspace
-                  reinterpret_cast<float*>(out)[size_t(ks) * n_tokens * out_stride + idx] = v;
-                else if constexpr (EPI == kEpiPushRS) {    // reduce-scatter by address into the row owner's slot
-                  const uint32_t owner = t / tp.rpr, tl = t - owner * tp.rpr;
-                  st_peer_bf16(reinterpret_cast<__nv_bfloat16*>(s_peer_slot[owner]) +
-                                   (size_t(tp.ctx.rank * split_k + ks) * tp.rpr + tl) * out_stride + n, v);
-                } else {
-                  if (split_k > 1) atomicAdd(reinterpret_cast<float*>(out) + idx, v);
-                  else reinterpret_cast<float*>(out)[idx] += v;
-                }
-              }
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar + acc);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      tc_epilogue<BN, EPI>(acc, out, mt * kBM + wrow, t0, n_tokens, n_out, out_stride, ks, split_k, tp, s_peer_slot, ep_ll);
     }
   }
 
   if (tb.data) {
     if (warp == 0 && lane == 0) stall[0] = c_wait;
-    if (warp == 1 && lane == 0) stall[1] = c_wait;
-    if (warp == 4 && lane == 0) stall[2] = c_wait;  // epilogue warp 4: first column half
+    if (warp == 4 && lane == 0) stall[1] = c_wait;   // consumer warpgroup 1
+    if (warp == 8 && lane == 0) stall[2] = c_wait;   // consumer warpgroup 2
   }
-  tc_fence_before();
   __syncthreads();
   if (tb.data && threadIdx.x == 0)
     trace_emit(tb, (6ull << 60) | ((unsigned long long)EPI << 56) | ((unsigned long long)n_out << 32) | K, g_begin, g_begin, gtime_ns(), n_tokens);
@@ -382,12 +255,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
     trace_emit(tb, (2ull << 60) | ((unsigned long long)n_out << 32) | ((unsigned long long)EPI << 28) | K,
                (unsigned long long)(clock64() - c_begin), (unsigned long long)stall[0], (unsigned long long)stall[1],
                (unsigned long long)stall[2]);
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"(uint32_t(Cfg::kTmemCols))
-                 : "memory");
-  }
   if constexpr (EPI == kEpiPushRS) {
     const uint32_t slot = tp.coll & 1;
     tp_signal_when_grid_done(tp.ctx, &tp_flags(tp.ctx, tp.ctx.rank)->done[slot], gridDim.x, tp_epoch(tp.ctx, tp.coll),
@@ -565,7 +432,7 @@ int gemm_tc2_launch(const CUtensorMap& tw, const CUtensorMap& tx_half, void* out
 // enough for 256-token tiles the CTA-pair kernel (gemm_tc2.cu) runs instead.
 // K-split (kEpiPartialF32 / kEpiPushRS / RESID_F32 only) up to max_split parts; *n_parts = parts used.
 // (A stream-K work split of the same pipeline was built and measured in round 1 — no better than
-// slab tiles + K-split partials in either regime; it lives in tools/experiments/csrc/gemm_sk.cu.)
+// slab tiles + K-split partials in either regime.)
 int gemm_tc_launch(const CUtensorMap& tw, const CUtensorMap& tx, void* out, uint32_t n_tokens,
                    uint32_t n_out, uint32_t k, uint32_t epi, uint32_t out_stride,
                    cudaStream_t st, const CUtensorMap* tx_half, uint32_t* n_parts,
@@ -604,8 +471,8 @@ int gemm_tc_launch(const CUtensorMap& tw, const CUtensorMap& tx, void* out, uint
 using namespace llmlb;
 
 // Kernel-level entry point of the tensor-core projections (parity tests, micro-benchmarks).
-// impl 0 = tcgen05 + TMEM + TMA tiles.  The mma.sync baseline (1) and the stream-K split (2) of
-// round 1 are no longer part of the library (tools/experiments/csrc/).
+// impl 0 = wgmma + TMA tiles.  The mma.sync baseline (1) and the stream-K split (2) of
+// round 1 are no longer part of the library.
 extern "C" int llmlb_op_gemm(const void* w, const void* x, void* out, uint32_t n_tokens,
                              uint32_t n_out, uint32_t k, uint32_t epilogue, uint32_t out_stride,
                              uint32_t impl, void* stream) {
@@ -628,7 +495,7 @@ extern "C" int llmlb_op_gemm(const void* w, const void* x, void* out, uint32_t n
     return LLMLB_E_INVALID_ARG;
   }
   if (impl != 0) {
-    set_error("llmlb_op_gemm: only impl 0 (tcgen05 tiles) is built into the library");
+    set_error("llmlb_op_gemm: only impl 0 (wgmma tiles) is built into the library");
     return LLMLB_E_UNSUPPORTED;
   }
   if (n_tokens == 0) return LLMLB_OK;

@@ -287,8 +287,8 @@ extern "C" int llmlb_op_gemv(const void* w, const void* x, const void* gain, flo
   }
   if (n_tokens >= 1 && n_tokens <= 4 && epilogue <= LLMLB_EPI_STORE_F32) {
     // K-split kernel (gemv_ks.cu) for every shape it takes; the row-owner kernel below is the
-    // fallback for odd K.  (A bulk-copy shared-memory ring variant was measured at 0.67 of HBM peak
-    // against 0.97 here and lives in tools/experiments/csrc/gemv_bulk.cu.)
+    // fallback for odd K.  (A bulk-copy shared-memory ring variant measured slower in round 1 and is not
+    // part of the library.)
     int rc = gemv_ks_try(w, x, gain, eps, out, n_tokens, n_out, k, epilogue, out_stride, st);
     if (rc != LLMLB_E_UNSUPPORTED) return rc;
   }

@@ -2,7 +2,7 @@
 //
 // Why: with "a warp owns whole rows" the work quantum is a 4-row group, and 7168 groups over
 // 2368 resident warps leaves some warps 4 trips and most 3 (25% tail), while N=4096 outputs only
-// fill 64 CTAs.  Here the quantum is one row PAIR per CTA: rows are dealt to the 148 CTAs in
+// fill 64 CTAs.  Here the quantum is one row PAIR per CTA: rows are dealt to the 132 CTAs in
 // contiguous, near-equal ranges and every warp of a CTA streams its own K slice of EVERY row of
 // the CTA, so all SMs pull from HBM for the whole kernel regardless of N.
 //   * CTA = 16 warps.  K is cut into 256-element chunks (one 16-byte load per lane); a "team" of
@@ -150,7 +150,7 @@ gemv_ks_kernel(const __nv_bfloat16* __restrict__ W, const void* xin /* predecess
       };
       if (tp.gather) {
         // (1) OWNER FOLD.  float4 i of every row belongs to CTA i % gridDim.x: only that CTA reads the N pushed
-        // partials (every CTA folding the whole residual costs 148 x N x K x 8 B of L2 reads per launch: 39 MB at
+        // partials (every CTA folding the whole residual costs 132 x N x K x 8 B of L2 reads per launch: 35 MB at
         // N = 8), writes the new residual and publishes it to the rest of the grid as {value, epoch} pairs.
         for (uint32_t i = blockIdx.x + gridDim.x * threadIdx.x; i < K / 4; i += gridDim.x * kKsThreads) {
 #pragma unroll

@@ -13,7 +13,7 @@
 
 namespace llmlb {
 
-constexpr int kArMaxBlocks = 148;
+constexpr int kArMaxBlocks = kNumSMs;
 static __device__ TraceBuf d_trace_tp;
 void tp_set_trace(const TraceBuf& tb) { cudaMemcpyToSymbol(d_trace_tp, &tb, sizeof(tb)); }
 

@@ -116,7 +116,7 @@ def lib():
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise FileNotFoundError(
-                LIB_PATH + " is missing: run `python -m llmlb_b200.build` (nvcc, sm_100a). "
+                LIB_PATH + " is missing: run `python -m llmlb_b200.build` (nvcc, sm_90a). "
                 "There is no CPU implementation of this path.")
         L = C.CDLL(LIB_PATH, mode=C.RTLD_GLOBAL)
         for name, (res, args) in PROTOTYPES.items():

@@ -483,7 +483,7 @@ static void handle(int fd, const Request& rq) {
     Json root = Json::object(); root.set("object", "list"); root.set("data", data);
     send_json(fd, 200, root.dump());
   } else if (rq.method == "GET" && path == "/api/system") {
-    Json root = Json::object(); root.set("xllm_version", "llmlb_b200-0.1"); root.set("engine", "llmlb_b200"); root.set("device", "NVIDIA B200");
+    Json root = Json::object(); root.set("xllm_version", "llmlb_b200-0.1"); root.set("engine", "llmlb_b200"); root.set("device", "NVIDIA H100");
     send_json(fd, 200, root.dump());
   } else if (rq.method == "GET" && path == "/api/health") {
     llmlb_health h; llmlb_engine_health(G.eng, &h);

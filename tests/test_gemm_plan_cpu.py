@@ -1,6 +1,6 @@
 """Host-side invariants of the in-kernel K-split of the store-epilogue GEMMs (llmlb_b200/csrc/gemm_tc.cu), without a GPU.
 The kernel's parts MEET at a counter and each finishes a share of the tile, so a launch is only correct when
-  * every CTA of the grid is resident at once: tiles x parts <= 148 (one tile per CTA, one CTA per SM),
+  * every CTA of the grid is resident at once: tiles x parts <= 132 (one tile per CTA, one CTA per SM),
   * every part owns at least one K block (an empty part would publish an untouched accumulator),
   * the parts cover K exactly with ceil(K blocks / parts) blocks each,
   * the parked tiles fit the workspace and the counters.
@@ -11,7 +11,7 @@ import random
 
 from llmlb_b200 import ffi
 
-SMS, BM, BK, WS_BYTES, COUNTERS = 148, 128, 64, 148 * 128 * 256 * 4, 256
+SMS, BM, BK, WS_BYTES, COUNTERS = 132, 128, 64, 132 * 128 * 256 * 4, 256
 
 
 def plan(L, T, N, K):
@@ -51,7 +51,7 @@ def test_shard_shapes_of_the_benchmark_models():
                     seen_split += check(L, T, n_out, k) > 1
     assert seen_split > 40      # the sweep does exercise the split (tp shards, narrow steps)
     # the cases quoted in DESIGN.md
-    assert plan(L, 64, 6144, 4096)[2] == 3          # QKV at 64 streams: 48 tiles -> 144 CTAs
+    assert plan(L, 64, 6144, 4096)[2] == 2          # QKV at 64 streams: 48 tiles -> 96 CTAs
     assert plan(L, 128, 768, 4096)[2:] == (16, 96)  # QKV at tp = 8, 128 streams
     assert plan(L, 64, 28672, 4096)[2] == 1         # gate/up at 64 streams: 224 tiles, no split
 

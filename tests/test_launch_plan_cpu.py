@@ -4,7 +4,7 @@ CUDA runtime and logs every kernel launch for EVERY prefill width 1..2048 and de
 
   * co-residency: kernels whose CTAs wait for each other inside the grid (the in-kernel K-split of gemm_tc / gemm_tc2 parks
     partial tiles and spins on a per-tile counter; the gemv_ks gather variant waits for owner CTAs) must fit the GPU in one
-    wave — at most 148 CTAs at one CTA per SM.  A wider grid would hang the device; GPU tests only ever try a few widths.
+    wave — at most 132 CTAs at one CTA per SM.  A wider grid would hang the device; GPU tests only ever try a few widths.
   * hardware limits: <= 1024 threads per CTA, <= 227 KiB dynamic shared memory, cluster size <= 16 and grid divisible by it.
   * every launch with more than 48 KiB of dynamic shared memory was preceded by the opt-in for THAT kernel function (each
     template instantiation needs its own cudaFuncSetAttribute; a missing one only fails at the widths that pick it) — the
@@ -25,7 +25,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 import test_engine_host_logic_cpu as HL  # noqa: E402
 
-SM_COUNT, MAX_SMEM = 148, 227 * 1024
+SM_COUNT, MAX_SMEM = 132, 227 * 1024
 MANGLED = {}
 
 

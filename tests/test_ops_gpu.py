@@ -149,7 +149,7 @@ def test_gemm_ksplit_back_to_back_is_bit_reproducible(L):
 
 
 def test_gemm_other_impls_are_not_in_the_library(L):
-    """The mma.sync baseline and the stream-K split of round 1 moved to tools/experiments/: asking for
+    """The mma.sync baseline and the stream-K split of round 1 are not part of the library: asking for
     them fails loudly instead of silently running something else."""
     w = bf16_randn((128, 64), std=0.02, seed=1)
     x = bf16_randn((16, 64), seed=2)

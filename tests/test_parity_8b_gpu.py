@@ -24,8 +24,7 @@ pytestmark = pytest.mark.gpu
 
 N_PROMPTS = int(os.environ.get("LLMLB_PARITY_PROMPTS", "8"))
 PROMPT, STEPS = 512, 32
-# Measured on B200 (round 2, 2 prompts): max|dlogit| 0.200, mean|dlogit| 0.0251, top-1 agreement 57/64
-# under teacher forcing, at a logit standard deviation of 1.28 — the synthetic N(0, 0.02^2) weights give
+# Logit standard deviation here is about 1.28 — the synthetic N(0, 0.02^2) weights give
 # very flat distributions (the top two of 128256 logits are typically ~0.1 apart), so arg-max flips at
 # near-ties are the common case and TOKEN IDENTITY is not the criterion: every token the engine picks
 # must be within NEAR_TIE of the oracle's arg-max logit.  Bounds = measured + margin.

@@ -45,7 +45,7 @@ def _bits(seed=2):
 
 def test_dry_run_single_gguf_takes_head_dim_from_the_q_projection(server_bin, tmp_path):
     """The file has hidden 512 and 8 heads of 128 and no attention.key_length: hidden / heads = 64 is
-    the wrong head width (this is what failed on the B200 in round 1)."""
+    the wrong head width (this is what failed on the GPU in round 1)."""
     import json
     pytest.importorskip("gguf")
     from gguf_util import write_tiny_llama_gguf

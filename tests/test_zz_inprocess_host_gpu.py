@@ -1,4 +1,4 @@
-"""examples/inprocess_host.c against the REAL engine on a B200: a C99 host over the three public headers serving the
+"""examples/inprocess_host.c against the REAL engine on an H100: a C99 host over the three public headers serving the
 gateway's hot path in-process (gate -> TPS router -> lease -> submit/poll -> SSE -> relay accounting -> TPS update), no HTTP.
 Checked two ways: the gateway oracle over the client-visible bytes and the router state (as in the CPU test against the
 scripted engine), and token-for-token against the Python ctypes host driving the same library with the same prompts.

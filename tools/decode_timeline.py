@@ -35,7 +35,7 @@ def main():
     for tag in np.unique(r[:, 0]):
         rows = r[r[:, 0] == tag]
         rows = rows[np.argsort(rows[:, 5])]
-        grid = 128 if int(tag) == 1 else 148
+        grid = 128 if int(tag) == 1 else 132
         for i in range(0, len(rows) - grid + 1, grid):
             blk = rows[i:i + grid]
             launches.append({"tag": int(tag), "rows": list(blk), "mid": float(np.median(blk[:, 5].astype(np.float64)))})

@@ -1,6 +1,6 @@
-"""Where the tcgen05 prefill GEMM's cycles go (debug hook llmlb_debug_trace_*): per kernel type,
-the share of CTA lifetime the TMA producer waited for a free smem slot, the MMA issuer waited for
-data, and the epilogue waited for a finished accumulator.  Run with LLMLB_GEMM_NO_2CTA=1 (the 1-CTA
+"""Where the wgmma prefill GEMM's cycles go (debug hook llmlb_debug_trace_*): per kernel type,
+the share of CTA lifetime the TMA producer waited for a free smem slot and each of the two consumer
+warpgroups waited for data.  Run with LLMLB_GEMM_NO_2CTA=1 (the 1-CTA
 kernel is the instrumented one)."""
 import ctypes as C
 import os
@@ -32,7 +32,7 @@ def main():
     r = buf[: n.value]
     r = r[(r[:, 0] >> np.uint64(60)) == 2]
     names = {0: "store_bf16", 1: "resid_f32", 2: "silu_mul", 3: "store_f32"}
-    print("%-34s %6s %10s %9s %9s %9s" % ("kernel", "ctas", "cycles", "prod_wait", "mma_wait", "epi_wait"))
+    print("%-34s %6s %10s %9s %9s %9s" % ("kernel", "ctas", "cycles", "prod_wait", "wg1_wait", "wg2_wait"))
     for tag in np.unique(r[:, 0]):
         rows = r[r[:, 0] == tag].astype(np.float64)
         t = int(tag)

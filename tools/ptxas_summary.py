@@ -7,7 +7,7 @@ import sys
 def main(path, pat=""):
     txt = open(path).read()
     rows = []
-    for m in re.finditer(r"Compiling entry function '(\S+)' for 'sm_100a'\n(?:.*\n)*?.*Used (\d+) registers(.*)", txt):
+    for m in re.finditer(r"Compiling entry function '(\S+)' for 'sm_90a'\n(?:.*\n)*?.*Used (\d+) registers(.*)", txt):
         name, regs, rest = m.group(1), int(m.group(2)), m.group(3)
         rows.append((name, regs, rest))
     if not rows:

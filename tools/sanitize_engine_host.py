@@ -37,7 +37,7 @@ def main():
     with ThreadPoolExecutor(max_workers=8) as ex:
         objs = list(ex.map(comp, B.SOURCES))
     lib = os.path.join(out, "libllmlb_b200.so")
-    subprocess.check_call([B.NVCC, "-shared", "-o", lib, *objs, "-gencode", "arch=compute_100a,code=sm_100a", *host, "-lcudart", "-lpthread"])
+    subprocess.check_call([B.NVCC, "-shared", "-o", lib, *objs, "-gencode", "arch=compute_90a,code=sm_90a", *host, "-lcudart", "-lpthread"])
     # the HTTP shim over the same library, same sanitizer
     hd = os.path.join(ROOT, "llmlb_b200", "host")
     server = os.path.join(out, "llmlb_b200_server")

@@ -120,7 +120,7 @@ def main():
         print("tp=%d geom=8b4 proto=%d max|dlogit| vs tp=1 engine: prefill512 %.4g decode %.4g %.4g prefill3 %.4g decode %.4g (logit std %.3f); "
               "ranks identical: %s; staggered requests token-identical to tp=1: %d/3; worst margin of a batched-step token to the tp=1 arg-max %.4f; lengths ok: %s"
               % (world, args.proto, d[0], d[1], d[2], d[3], d[4], float(l1.std()), same, eq3, worst, lens_ok))
-        # measured on B200: 0.062 (tp=2), 0.072 (tp=8) on prefill512 at a logit std of 1.28 (bf16 partials on the wire, N-way order)
+        # bound on prefill512 at a logit std of about 1.28 (bf16 partials on the wire, N-way order)
         ok = max(d) < 0.10 and same and lens_ok and worst < 0.2
     elif rank == 0:
         from oracle.llama_ref import LlamaRef
