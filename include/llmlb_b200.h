@@ -230,6 +230,13 @@ int llmlb_op_gemv(const void* w_bf16, const void* x, const void* gain_bf16, floa
 int llmlb_op_gemm(const void* w_bf16, const void* x_bf16, void* out, uint32_t n_tokens,
                   uint32_t n_out, uint32_t k, uint32_t epilogue, uint32_t out_stride,
                   uint32_t impl, void* stream);
+/* The same projection as the engine issues it, for kernel tests.  epilogue 4 = fp32 K-split partials: part ks at
+ * out_f32 + ks*n_tokens*out_stride, *n_parts = parts written (the consumer sums them in part order).  Rows
+ * [row0, row0 + n_rows) of W only (n_rows = 0: all; row0 a multiple of 256), as the wave-tail pair of launches does.
+ * max_split (1..16) bounds the K-split of the residual and partial epilogues. */
+int llmlb_debug_gemm(const void* w_bf16, const void* x_bf16, void* out, uint32_t n_tokens, uint32_t n_out, uint32_t k,
+                     uint32_t epilogue, uint32_t out_stride, uint32_t row0, uint32_t n_rows, uint32_t max_split,
+                     uint32_t* n_parts, void* stream);
 
 /* RoPE table: fp32 (cos, sin) pairs [max_pos][64] for head_dim 128, HF rotate-half pairing. */
 int llmlb_op_rope_table(float* table, uint32_t max_pos, float theta, void* stream);

@@ -470,6 +470,19 @@ int gemm_tc_launch(const CUtensorMap& tw, const CUtensorMap& tx, void* out, uint
 
 using namespace llmlb;
 
+// The kernel-level entry points own one K-split workspace per process (callers are serialised tests / benches).
+static int op_split_workspace(TpPushRS* tpp) {
+  static float* op_ws = nullptr;
+  static unsigned int* op_cnt = nullptr;
+  if (!op_ws) {
+    LLMLB_CUDA_CHECK(cudaMalloc((void**)&op_ws, kSkWsBytes));
+    LLMLB_CUDA_CHECK(cudaMalloc((void**)&op_cnt, kSkCounters * sizeof(unsigned int)));
+    LLMLB_CUDA_CHECK(cudaMemset(op_cnt, 0, kSkCounters * sizeof(unsigned int)));
+  }
+  tpp->sk_ws = op_ws; tpp->sk_cnt = op_cnt;
+  return LLMLB_OK;
+}
+
 // Kernel-level entry point of the tensor-core projections (parity tests, micro-benchmarks).
 // impl 0 = wgmma + TMA tiles.  The mma.sync baseline (1) and the stream-K split (2) of
 // round 1 are no longer part of the library.
@@ -507,17 +520,40 @@ extern "C" int llmlb_op_gemm(const void* w, const void* x, void* out, uint32_t n
   if (rc) return rc;
   rc = make_tmap_bf16(&txh, x, n_tokens, k, 128);
   if (rc) return rc;
-  // the kernel-level entry point owns one K-split workspace per process (callers are serialised tests / benches)
-  static float* op_ws = nullptr;
-  static unsigned int* op_cnt = nullptr;
-  if (!op_ws) {
-    LLMLB_CUDA_CHECK(cudaMalloc((void**)&op_ws, kSkWsBytes));
-    LLMLB_CUDA_CHECK(cudaMalloc((void**)&op_cnt, kSkCounters * sizeof(unsigned int)));
-    LLMLB_CUDA_CHECK(cudaMemset(op_cnt, 0, kSkCounters * sizeof(unsigned int)));
-  }
   TpPushRS tpp{};
-  tpp.sk_ws = op_ws; tpp.sk_cnt = op_cnt;
+  rc = op_split_workspace(&tpp);
+  if (rc) return rc;
   return gemm_tc_launch(tw, tx, out, n_tokens, n_out, k, epilogue, out_stride, st, &txh, nullptr, &tpp, 8);
+}
+
+// The projection as the engine issues it, for kernel tests: the internal fp32 K-split partial epilogue (epi 4: part ks
+// at out + ks * n_tokens * out_stride, *n_parts = parts written) and the row window [row0, row0 + n_rows) of W that a
+// wave-tail launch covers (n_rows = 0: all rows; row0 a multiple of 256).  max_split bounds the K-split of the
+// residual / partial epilogues as in the engine (1..16).
+extern "C" int llmlb_debug_gemm(const void* w, const void* x, void* out, uint32_t n_tokens, uint32_t n_out, uint32_t k,
+                                uint32_t epilogue, uint32_t out_stride, uint32_t row0, uint32_t n_rows, uint32_t max_split,
+                                uint32_t* n_parts, void* stream) {
+  if (!w || !x || !out || n_out == 0 || k == 0 || k % 8 != 0 || n_tokens > (1u << 20) || n_out > (1u << 24) ||
+      k > (1u << 20) || epilogue > uint32_t(kEpiPartialF32) || (epilogue == LLMLB_EPI_SILU_MUL && (n_out & 1)) ||
+      row0 % 256 != 0 || (n_rows == 0 && row0 != 0) || uint64_t(row0) + n_rows > n_out || max_split == 0 || max_split > 16) {
+    set_error("llmlb_debug_gemm: bad argument");
+    return LLMLB_E_INVALID_ARG;
+  }
+  if (n_parts) *n_parts = 0;
+  if (n_tokens == 0) return LLMLB_OK;
+  CUtensorMap tw, tx, txh;
+  int rc = make_tmap_bf16(&tw, w, n_out, k, 128);
+  if (rc) return rc;
+  rc = make_tmap_bf16(&tx, x, n_tokens, k, tc_pick_bn(n_tokens));
+  if (rc) return rc;
+  rc = make_tmap_bf16(&txh, x, n_tokens, k, 128);
+  if (rc) return rc;
+  TpPushRS tpp{};
+  rc = op_split_workspace(&tpp);
+  if (rc) return rc;
+  tpp.row0 = row0; tpp.n_rows = n_rows;
+  return gemm_tc_launch(tw, tx, out, n_tokens, n_out, k, epilogue, out_stride, (cudaStream_t)stream, &txh, n_parts, &tpp,
+                        max_split);
 }
 
 // Host-only (no launch, no device): the K-split a store-epilogue projection of this shape would run with, and the grid

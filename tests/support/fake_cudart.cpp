@@ -208,14 +208,18 @@ cudaError_t cudaGraphDestroy(cudaGraph_t g) { free(g); return cudaSuccess; }
 cudaError_t cudaGraphExecDestroy(cudaGraphExec_t x) { free(x); return cudaSuccess; }
 // FAKE_CUDART_LAUNCH_LOG=<file>: one line per kernel launch — mangled kernel name, grid, block, dynamic shared memory,
 // cluster dims and whether it was launched as a programmatic dependent (PDL) — the engine's LAUNCH PLAN for any geometry,
-// readable without a GPU (tests/test_launch_plan_cpu.py checks co-residency and resource limits on it).
-static void log_launch(const void* fn, dim3 g, dim3 b, size_t smem, dim3 cluster, int pdl) {
+// readable without a GPU (tests/test_launch_plan_cpu.py checks co-residency and resource limits on it).  Launches of the
+// projection GEMMs (gemm_tc_kernel / gemm_tc2_kernel, whose 10th parameter is split_k) append that K-split count, so that
+// tests/test_kernel_coverage_cpu.py can tell a K-split launch from a plain one.
+static void log_launch(const void* fn, dim3 g, dim3 b, size_t smem, dim3 cluster, int pdl, void** args = nullptr) {
   static FILE* f = getenv("FAKE_CUDART_LAUNCH_LOG") ? fopen(getenv("FAKE_CUDART_LAUNCH_LOG"), "a") : nullptr;
   if (!f) return;
   std::lock_guard<std::mutex> lk(g_mu);
   auto it = g_kernels.find(fn);
-  fprintf(f, "%s %u %u %u %u %u %u %zu %u %u %u %d\n", it == g_kernels.end() ? "?" : it->second.c_str(), g.x, g.y, g.z, b.x, b.y, b.z, smem,
-          cluster.x, cluster.y, cluster.z, pdl);
+  const char* name = it == g_kernels.end() ? "?" : it->second.c_str();
+  fprintf(f, "%s %u %u %u %u %u %u %zu %u %u %u %d", name, g.x, g.y, g.z, b.x, b.y, b.z, smem, cluster.x, cluster.y, cluster.z, pdl);
+  if (args && (strstr(name, "gemm_tc_kernel") || strstr(name, "gemm_tc2_kernel"))) fprintf(f, " %u", *static_cast<const uint32_t*>(args[9]));
+  fputc('\n', f);
   fflush(f);
 }
 cudaError_t cudaLaunchKernel(const void* fn, dim3 g, dim3 b, void**, size_t smem, cudaStream_t) {
@@ -225,7 +229,7 @@ cudaError_t cudaLaunchKernel(const void* fn, dim3 g, dim3 b, void**, size_t smem
   log_launch(fn, g, b, smem, dim3(1, 1, 1), 0);
   return cudaSuccess;
 }
-cudaError_t cudaLaunchKernelExC(const cudaLaunchConfig_t* c, const void* fn, void**) {
+cudaError_t cudaLaunchKernelExC(const cudaLaunchConfig_t* c, const void* fn, void** args) {
   if (!config_allowed(c->gridDim, c->blockDim)) return g_last_error = cudaErrorInvalidConfiguration;
   if (!smem_allowed(fn, c->dynamicSmemBytes)) return g_last_error = cudaErrorInvalidValue;
   ++g_launches;
@@ -235,7 +239,7 @@ cudaError_t cudaLaunchKernelExC(const cudaLaunchConfig_t* c, const void* fn, voi
     if (c->attrs[i].id == cudaLaunchAttributeClusterDimension) cluster = dim3(c->attrs[i].val.clusterDim.x, c->attrs[i].val.clusterDim.y, c->attrs[i].val.clusterDim.z);
     if (c->attrs[i].id == cudaLaunchAttributeProgrammaticStreamSerialization) pdl = c->attrs[i].val.programmaticStreamSerializationAllowed;
   }
-  log_launch(fn, c->gridDim, c->blockDim, c->dynamicSmemBytes, cluster, pdl);
+  log_launch(fn, c->gridDim, c->blockDim, c->dynamicSmemBytes, cluster, pdl, args);
   return cudaSuccess;
 }
 // More than 48 KiB of dynamic shared memory needs an opt-in per kernel FUNCTION (each template instantiation is its own):
