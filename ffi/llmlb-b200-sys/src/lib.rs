@@ -137,6 +137,7 @@ extern "C" {
     pub fn llmlb_engine_model_info(e: *const llmlb_engine, out: *mut llmlb_model_info) -> c_int;
     pub fn llmlb_engine_health(e: *const llmlb_engine, out: *mut llmlb_health) -> c_int;
     pub fn llmlb_engine_load_tensor(e: *mut llmlb_engine, name: *const c_char, host_bf16: *const u8, rows: u64, cols: u64) -> c_int;
+    pub fn llmlb_engine_set_rope_freq_factors(e: *mut llmlb_engine, factors: *const f32, n: u32) -> c_int;
     pub fn llmlb_engine_tp_export(e: *mut llmlb_engine, handle: *mut u8) -> c_int;
     pub fn llmlb_engine_tp_import(e: *mut llmlb_engine, handles: *const u8, n: u32) -> c_int;
     pub fn llmlb_engine_tp_plan_channel(e: *mut llmlb_engine, shm_name: *const c_char) -> c_int;
@@ -251,6 +252,11 @@ impl Engine {
             tp_proto: 0,
             reserved: [0; 3],
         }
+    }
+
+    /// RoPE frequency scaling (llama3 / linear): 64 per-frequency divisors, before the first request.
+    pub fn set_rope_freq_factors(&self, factors: &[f32]) -> Result<(), EngineError> {
+        check(unsafe { llmlb_engine_set_rope_freq_factors(self.raw, factors.as_ptr(), factors.len() as u32) })
     }
 
     pub fn submit(&self, prompt_ids: &[i32], s: &Sampling) -> Result<u64, EngineError> {

@@ -115,6 +115,11 @@ int llmlb_engine_tp_plan_channel(llmlb_engine* e, const char* shm_name);
  * checkpoint: "model.embed_tokens.weight", "model.layers.N.self_attn.q_proj.weight", ... */
 int llmlb_engine_load_tensor(llmlb_engine* e, const char* name, const void* host_bf16,
                              uint64_t rows, uint64_t cols);
+/* RoPE frequency scaling (llama3 / linear, as GGUF's rope_freqs.weight carries it): rebuild this rank's RoPE table with
+ * inv_freq[j] = theta^(-2j/128) / factors[j].  n must be head_dim/2 (64); every factor finite and > 0, else
+ * LLMLB_E_INVALID_ARG.  Only before the first request or debug call (LLMLB_E_UNSUPPORTED after: no running sequence
+ * may see its positions change meaning).  With tensor parallelism every rank calls it. */
+int llmlb_engine_set_rope_freq_factors(llmlb_engine* e, const float* factors, uint32_t n);
 /* Copy this rank's slice of a tensor back to the host as bf16 (debug / CPU-baseline feed).
  * name as above; returns rows/cols of the slice. cap_bytes guards the buffer. */
 int llmlb_engine_read_tensor(llmlb_engine* e, const char* name, void* host_bf16,
@@ -240,6 +245,10 @@ int llmlb_debug_gemm(const void* w_bf16, const void* x_bf16, void* out, uint32_t
 
 /* RoPE table: fp32 (cos, sin) pairs [max_pos][64] for head_dim 128, HF rotate-half pairing. */
 int llmlb_op_rope_table(float* table, uint32_t max_pos, float theta, void* stream);
+/* The same with per-frequency divisors (llama3 / linear RoPE scaling, GGUF rope_freqs.weight):
+ * angle = pos * theta^(-2j/128) / factors[j], in fp64.  factors: host, 64 floats, each finite and > 0; NULL = none
+ * (bit-identical to llmlb_op_rope_table, as is a table of 1.0s). */
+int llmlb_op_rope_table_scaled(float* table, uint32_t max_pos, float theta, const float* factors, void* stream);
 /* KV pages: K and V pools are [page][kv_head][64 tokens][128] bf16.
  * a2.4+a2.5 prefill: rotate q,k in place inside qkv [t, (nq+2nkv)*128] and append k,v to pages.
  * page_of_token[t] = page holding positions[t] (negative = do not append). */

@@ -135,6 +135,10 @@ uint32_t llmlb_ckpt_count(void* ckpt);
 int llmlb_ckpt_is_gguf(void* ckpt);
 /* u7: hidden, n_layers, n_heads, n_kv_heads, head_dim, ffn, vocab; f2: rope_theta, rms_eps.  1 = geometry complete */
 int llmlb_ckpt_geometry(void* ckpt, uint32_t* u7, float* f2);
+/* RoPE frequency scaling the file states (GGUF rope_freqs.weight / linear metadata, llama3 or linear in a config.json
+ * beside a safetensors file): per-frequency divisors, up to cap of them written to out.  Returns how many there are
+ * (head_dim/2), 0 = no scaling. */
+uint32_t llmlb_ckpt_rope_freq_factors(void* ckpt, float* out, uint32_t cap);
 int64_t llmlb_ckpt_tensor_info(void* ckpt, uint32_t index, char* name, uint32_t name_cap, uint64_t* rows, uint64_t* cols);   /* element count, -1 bad index */
 int llmlb_ckpt_tensor_bf16(void* ckpt, uint32_t index, uint16_t* out, uint64_t cap_elems);
 int64_t llmlb_ckpt_tokenizer_json(void* ckpt, char* out, uint64_t cap);                   /* GGUF tokenizer.ggml.* as tokenizer.json text */

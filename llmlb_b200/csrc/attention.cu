@@ -17,11 +17,18 @@ namespace llmlb {
 
 constexpr float kLog2e = 1.4426950408889634f;
 
-__global__ void rope_table_kernel(float2* __restrict__ table, uint32_t max_pos, double theta) {
+// Per-frequency RoPE divisors (llama3 / linear scaling, GGUF rope_freqs): inv_freq[j] = theta^(-2j/128) / f[j].
+struct RopeFactors {
+  float f[64];
+};
+
+// Angles in fp64.  A divisor of exactly 1.0 leaves inv unchanged (exact in fp64), so an unscaled table is
+// bit-identical to one built without divisors.
+__global__ void rope_table_kernel(float2* __restrict__ table, uint32_t max_pos, double theta, RopeFactors fac) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= max_pos * 64) return;
   uint32_t pos = i / 64, j = i % 64;
-  double inv = pow(theta, -double(2 * j) / double(kHeadDim));
+  double inv = pow(theta, -double(2 * j) / double(kHeadDim)) / double(fac.f[j]);
   double a = double(pos) * inv;
   table[i] = make_float2(float(cos(a)), float(sin(a)));
 }
@@ -598,16 +605,29 @@ decode_attention_kernel(const __nv_bfloat16* qkv /* NOT __restrict__: written by
 
 using namespace llmlb;
 
-extern "C" int llmlb_op_rope_table(float* table, uint32_t max_pos, float theta, void* stream) {
+extern "C" int llmlb_op_rope_table_scaled(float* table, uint32_t max_pos, float theta, const float* factors,
+                                          void* stream) {
   if (!table || max_pos == 0) {
     set_error("llmlb_op_rope_table: bad argument");
     return LLMLB_E_INVALID_ARG;
   }
+  RopeFactors fac;
+  for (int j = 0; j < 64; ++j) {
+    fac.f[j] = factors ? factors[j] : 1.f;
+    if (!(fac.f[j] > 0.f) || !std::isfinite(fac.f[j])) {
+      set_error("llmlb_op_rope_table_scaled: every factor must be finite and > 0");
+      return LLMLB_E_INVALID_ARG;
+    }
+  }
   uint32_t n = max_pos * 64;
   rope_table_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>((float2*)table, max_pos,
-                                                                       (double)theta);
+                                                                       (double)theta, fac);
   LLMLB_LAUNCH_CHECK();
   return LLMLB_OK;
+}
+
+extern "C" int llmlb_op_rope_table(float* table, uint32_t max_pos, float theta, void* stream) {
+  return llmlb_op_rope_table_scaled(table, max_pos, theta, nullptr, stream);
 }
 
 namespace llmlb {

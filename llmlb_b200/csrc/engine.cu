@@ -424,6 +424,7 @@ struct llmlb_engine {
   std::atomic<uint64_t> steps_prefill{0}, steps_decode{0}, tokens_prefill{0}, tokens_decode{0};
   double gpu_ms_prefill = 0, gpu_ms_decode = 0;  // under mu
   int debug_slot = -1;
+  std::atomic<bool> served{false};   // a request was submitted or a step / debug forward ran: the RoPE table is fixed
   std::vector<int32_t> debug_pages;
   uint32_t debug_len = 0;
 
@@ -498,6 +499,8 @@ struct llmlb_engine {
 };
 
 extern "C" int llmlb_op_rope_table(float* table, uint32_t max_pos, float theta, void* stream);
+extern "C" int llmlb_op_rope_table_scaled(float* table, uint32_t max_pos, float theta, const float* factors,
+                                          void* stream);
 extern "C" int llmlb_op_rope_append(void* qkv, const int32_t* positions,
                                     const int32_t* page_of_token, const float* rope_table,
                                     void* k_pages, void* v_pages, uint32_t n_tokens,
@@ -1054,6 +1057,7 @@ cudaEvent_t llmlb_engine::get_event() {
 int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector<uint32_t>& take) {
   uint32_t T = 0;
   for (uint32_t t : take) T += t;
+  served = true;   // a follower rank of a plan channel never sees the submit
   uint8_t* stg = next_stage();
   int32_t* s_ids = reinterpret_cast<int32_t*>(stg);
   int32_t* s_pos = s_ids + t_cap;
@@ -1619,6 +1623,7 @@ extern "C" int llmlb_request_submit(llmlb_engine* e, const int32_t* prompt_ids, 
     if (!e->fatal_error.empty()) { set_error("engine failed: " + e->fatal_error); return LLMLB_E_DEVICE; }
     if (e->waiting.size() >= (e->cfg.queue_max ? e->cfg.queue_max : 4096u)) { set_error("Request queue is full"); return LLMLB_E_QUEUE_FULL; }
     r->id = e->next_id++;
+    e->served = true;
     e->requests[r->id] = r;
     e->waiting.push_back(r);
     *req_id = r->id;
@@ -1855,6 +1860,28 @@ extern "C" int llmlb_engine_load_tensor(llmlb_engine* e, const char* name, const
   return LLMLB_OK;
 }
 
+extern "C" int llmlb_engine_set_rope_freq_factors(llmlb_engine* e, const float* factors, uint32_t n) {
+  if (!e || !factors) { set_error("llmlb_engine_set_rope_freq_factors: null argument"); return LLMLB_E_INVALID_ARG; }
+  if (n != uint32_t(kHeadDim / 2)) { set_error("llmlb_engine_set_rope_freq_factors: n must be head_dim/2 = 64"); return LLMLB_E_INVALID_ARG; }
+  for (uint32_t j = 0; j < n; ++j)
+    if (!std::isfinite(factors[j]) || !(factors[j] > 0.f)) {
+      set_error("llmlb_engine_set_rope_freq_factors: factor " + std::to_string(j) + " is not finite and > 0");
+      return LLMLB_E_INVALID_ARG;
+    }
+  cudaSetDevice(e->cfg.device);
+  std::lock_guard<std::mutex> sl(e->step_mu);
+  {
+    std::lock_guard<std::mutex> lk(e->mu);
+    if (e->served) {   // positions already in the KV cache were rotated with the old table
+      set_error("llmlb_engine_set_rope_freq_factors: only before the first request or debug call");
+      return LLMLB_E_UNSUPPORTED;
+    }
+  }
+  RC(llmlb_op_rope_table_scaled(e->rope, e->cfg.max_ctx, e->M.rope_theta, factors, e->st));
+  LLMLB_CUDA_CHECK(cudaStreamSynchronize(e->st));
+  return LLMLB_OK;
+}
+
 extern "C" int llmlb_engine_read_tensor(llmlb_engine* e, const char* name, void* host,
                                         uint64_t cap_bytes, uint64_t* rows, uint64_t* cols) {
   if (!e || !name || !host || !rows || !cols) { set_error("null argument"); return LLMLB_E_INVALID_ARG; }
@@ -1876,6 +1903,7 @@ static int debug_acquire(llmlb_engine* e) {  // step_mu held
     set_error("debug hooks need an idle engine");
     return LLMLB_E_QUEUE_FULL;
   }
+  e->served = true;
   if (e->debug_slot < 0) {
     if (e->free_slots.empty() || e->free_pages.size() < e->pages_per_seq) { set_error("no free slot/pages"); return LLMLB_E_QUEUE_FULL; }
     e->debug_slot = e->free_slots.back(); e->free_slots.pop_back();

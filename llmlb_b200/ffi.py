@@ -73,6 +73,7 @@ PROTOTYPES = {
     "llmlb_engine_tp_plan_channel": (C.c_int, [vp, cp]),
     "llmlb_engine_load_tensor": (C.c_int, [vp, cp, vp, u64, u64]),
     "llmlb_engine_read_tensor": (C.c_int, [vp, cp, vp, u64, _P(u64), _P(u64)]),
+    "llmlb_engine_set_rope_freq_factors": (C.c_int, [vp, _P(f32), u32]),
     "llmlb_engine_model_info": (C.c_int, [vp, _P(ModelInfo)]),
     "llmlb_engine_health": (C.c_int, [vp, _P(Health)]),
     "llmlb_engine_pause": (C.c_int, [vp, u32]),
@@ -91,6 +92,7 @@ PROTOTYPES = {
     "llmlb_op_gemm": (C.c_int, [vp, vp, vp, u32, u32, u32, u32, u32, u32, vp]),
     "llmlb_debug_gemm": (C.c_int, [vp, vp, vp, u32, u32, u32, u32, u32, u32, u32, u32, _P(u32), vp]),
     "llmlb_op_rope_table": (C.c_int, [vp, u32, f32, vp]),
+    "llmlb_op_rope_table_scaled": (C.c_int, [vp, u32, f32, _P(f32), vp]),
     "llmlb_op_rope_append": (C.c_int, [vp, vp, vp, vp, vp, vp, u32, u32, u32, vp]),
     "llmlb_op_prefill_attention": (C.c_int, [vp, vp, vp, vp, u32, vp, u32, vp, u32, u32, vp]),
     "llmlb_op_prefill_attention_tc": (C.c_int, [vp, u32, vp, vp, u32, vp, u32, vp, u32, vp, u32, u32, vp]),
@@ -158,7 +160,8 @@ class Engine:
 
     def __init__(self, model, model_id="llama-3-8b-synthetic", device=0, tp_rank=0, tp_size=1,
                  max_seqs=8, max_ctx=1024, kv_pages=0, max_step_tokens=0, seed=0,
-                 use_cuda_graphs=True, gemm_impl=0, lookahead=0, queue_max=0, queue_timeout_ms=0, request_timeout_ms=0, attn_impl=0, tp_proto=0):
+                 use_cuda_graphs=True, gemm_impl=0, lookahead=0, queue_max=0, queue_timeout_ms=0, request_timeout_ms=0, attn_impl=0, tp_proto=0,
+                 rope_freq_factors=None):
         cfg = EngineConfig()
         cfg.abi_version = ABI_VERSION
         for k, v in model.items():
@@ -176,6 +179,17 @@ class Engine:
         self.cfg = cfg
         self._h = vp()
         check(lib().llmlb_engine_create(C.byref(cfg), C.byref(self._h)))
+        if rope_freq_factors is not None:
+            try:
+                self.set_rope_freq_factors(rope_freq_factors)
+            except Exception:
+                self.close()
+                raise
+
+    def set_rope_freq_factors(self, factors):
+        """Per-frequency RoPE divisors (64 for head_dim 128); only before the first request or debug call."""
+        f = (f32 * max(1, len(factors)))(*[float(x) for x in factors])
+        check(lib().llmlb_engine_set_rope_freq_factors(self._h, f, len(factors)))
 
     def close(self):
         if self._h:

@@ -277,6 +277,45 @@ def geometry(meta, tensors):
             "rope_theta": float(g("rope.freq_base", 10000.0)), "rms_eps": float(g("attention.layer_norm_rms_epsilon", 1e-5))}
 
 
+def rope_scaling(meta, tensors, mm):
+    """RoPE frequency scaling a GGUF file states: (type, float32 divisors [head_dim/2] or None).
+    `rope_freqs.weight` (F32, what convert_hf_to_gguf.py writes for Llama 3.1+) is returned bit for bit
+    as type "rope_freqs"; `{arch}.rope.scaling.type = linear` multiplies every divisor by its factor;
+    "none" or no key is no scaling.  Any other type raises GGUFError."""
+    arch = meta.get("general.architecture", "llama")
+    n = geometry(meta, tensors)["head_dim"] // 2
+    kind, f = "none", None
+    rf = [t for t in tensors if t["name"] == "rope_freqs.weight"]
+    if rf:
+        t = rf[0]
+        if t["type"] != 0 or t["shape"] != [n] or n == 0:
+            raise GGUFError("rope_freqs.weight must be %d F32 values (head_dim / 2)" % n)
+        f = np.frombuffer(mm, dtype="<f4", count=n, offset=t["offset"]).astype(np.float32)
+        if not (np.isfinite(f).all() and (f > 0).all()):
+            raise GGUFError("rope_freqs.weight holds a factor that is not finite and > 0")
+        kind = "rope_freqs"
+    stype = meta.get(arch + ".rope.scaling.type")
+    if stype not in (None, "", "none"):
+        if stype != "linear":
+            raise GGUFError("unsupported RoPE scaling type %r: only linear and rope_freqs.weight are served" % (stype,))
+        factor = float(meta.get(arch + ".rope.scaling.factor", 0.0))
+        if not (np.isfinite(factor) and factor > 0):
+            raise GGUFError("RoPE scaling: factor must be finite and > 0")
+        lin = np.full(n, factor, dtype=np.float32)
+        f = lin if f is None else f * lin      # llama.cpp applies both
+        kind = "linear"
+    return kind, f
+
+
+def read_rope_scaling(path):
+    """rope_scaling() of the file at `path`."""
+    meta, tensors, mm = read_gguf(os.fspath(path))
+    try:
+        return rope_scaling(meta, tensors, mm)
+    finally:
+        mm.close()
+
+
 def iter_hf_tensors(path):
     """Yields (hf_name, bf16 bits [rows, cols]) for every tensor the engine can take, dequantised and
     with Q/K rows back in Hugging Face order.  A tied output head (no output.weight) is served

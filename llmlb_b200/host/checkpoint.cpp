@@ -9,7 +9,10 @@
 #include <sys/stat.h>
 #include <unistd.h>
 
+#include <cmath>
 #include <cstring>
+#include <fstream>
+#include <sstream>
 
 #include "json.hpp"
 
@@ -224,6 +227,38 @@ bool ggml_dequantize(uint32_t type, const uint8_t* src, size_t nbytes, float* ds
   return true;
 }
 
+bool rope_scaling_factors(const std::string& type, double factor, double low, double high, double old_ctx, double theta,
+                          uint32_t head_dim, std::vector<float>* out, std::string* err) {
+  out->clear();
+  if (type.empty() || type == "default" || type == "none") return true;
+  const uint32_t n = head_dim / 2;
+  if (type != "llama3" && type != "linear") {
+    if (err) *err = "unsupported RoPE scaling type '" + type + "': only llama3 and linear are served (dynamic, yarn and longrope "
+                    "depend on the sequence length or scale attention)";
+    return false;
+  }
+  if (!(factor > 0.0) || !std::isfinite(factor)) { if (err) *err = "RoPE scaling: factor must be finite and > 0"; return false; }
+  if (type == "linear") { out->assign(n, float(factor)); return true; }
+  if (!(low > 0.0) || !(high > low) || !std::isfinite(high) || !(old_ctx > 0.0) || !std::isfinite(old_ctx) || !(theta > 1.0)) {
+    if (err) *err = "RoPE scaling llama3: needs low_freq_factor > 0, high_freq_factor > low_freq_factor, original_max_position_embeddings > 0";
+    return false;
+  }
+  const double pi = 3.14159265358979323846;
+  for (uint32_t j = 0; j < n; ++j) {
+    const double inv = 1.0 / std::pow(theta, double(2 * j) / double(head_dim));
+    const double wavelen = 2 * pi / inv;
+    double f;
+    if (wavelen < old_ctx / high) f = 1.0;                 // high frequencies: unchanged
+    else if (wavelen > old_ctx / low) f = factor;          // low frequencies: divided by `factor`
+    else {                                                 // medium: interpolated
+      const double smooth = (old_ctx / wavelen - low) / (high - low);
+      f = 1.0 / ((1 - smooth) / factor + smooth);
+    }
+    out->push_back(float(f));
+  }
+  return true;
+}
+
 Checkpoint::~Checkpoint() { if (data_) munmap(const_cast<uint8_t*>(data_), size_); }
 
 bool Checkpoint::open(const std::string& path, std::string* err) {
@@ -235,6 +270,7 @@ bool Checkpoint::open(const std::string& path, std::string* err) {
   close(fd);
   if (p == MAP_FAILED) { if (err) *err = "mmap failed for " + path; return false; }
   data_ = static_cast<const uint8_t*>(p);
+  path_ = path;
   gguf_ = memcmp(data_, "GGUF", 4) == 0;
   return gguf_ ? open_gguf(err) : open_safetensors(err);
 }
@@ -286,6 +322,63 @@ bool Checkpoint::open_safetensors(std::string* err) {
   geo_.rope_theta = 500000.f;   // not stored in the tensor file (config.json): Llama-3 values, overridable by the caller
   geo_.rms_eps = 1e-5f;
   geo_.known = geo_.hidden && geo_.n_layers && geo_.n_heads && geo_.n_kv_heads && geo_.ffn && geo_.vocab;
+  return read_config_json(max_layer, err);
+}
+
+// The Hugging Face config.json beside a safetensors file: RoPE theta and scaling, RMSNorm eps, and the
+// geometry, which must agree with the tensor shapes this file holds.  Without one nothing changes.
+bool Checkpoint::read_config_json(int64_t max_layer, std::string* err) {
+  const size_t slash = path_.rfind('/');
+  const std::string cpath = (slash == std::string::npos ? std::string() : path_.substr(0, slash + 1)) + "config.json";
+  std::ifstream f(cpath, std::ios::binary);
+  if (!f) return true;
+  std::stringstream ss;
+  ss << f.rdbuf();
+  auto fail = [&](const std::string& m) { if (err) *err = cpath + ": " + m; return false; };
+  Json cfg;
+  if (!Json::parse(ss.str(), &cfg) || !cfg.is_object()) return fail("not a JSON object");
+  auto num = [](const Json* o, const char* k, double dflt) { const Json* v = o ? o->get(k) : nullptr; return v && v->is_number() ? v->as_double() : dflt; };
+  auto str = [](const Json* o, const char* k) { const Json* v = o ? o->get(k) : nullptr; return v && v->is_string() ? v->str() : std::string(); };
+  // geometry: every field the tensors of this file show must match
+  const double heads = num(&cfg, "num_attention_heads", 0), hidden = num(&cfg, "hidden_size", 0);
+  const double head_dim = num(&cfg, "head_dim", heads > 0 ? hidden / heads : 0);
+  if (heads > 0 && head_dim != 128) return fail("head_dim " + std::to_string(int64_t(head_dim)) + ": the engine serves head_dim 128 only");
+  struct { const char* key; double dflt; uint32_t seen; } checks[] = {
+      {"hidden_size", 0, geo_.hidden}, {"num_attention_heads", 0, geo_.n_heads}, {"num_key_value_heads", heads, geo_.n_kv_heads},
+      {"intermediate_size", 0, geo_.ffn}, {"vocab_size", 0, geo_.vocab}};
+  for (const auto& c : checks) {
+    const double v = num(&cfg, c.key, c.dflt);
+    if (c.seen && v > 0 && v != double(c.seen))
+      return fail(std::string(c.key) + " is " + std::to_string(int64_t(v)) + " but the tensor shapes say " + std::to_string(c.seen));
+  }
+  const double n_layers = num(&cfg, "num_hidden_layers", 0);
+  if (n_layers > 0) {
+    if (n_layers > double(kMaxLayers)) return fail("num_hidden_layers out of range");
+    if (max_layer >= int64_t(n_layers))
+      return fail("num_hidden_layers is " + std::to_string(int64_t(n_layers)) + " but the file holds layer " + std::to_string(max_layer));
+    geo_.n_layers = uint32_t(n_layers);
+  }
+  // RoPE: transformers 5 writes rope_parameters {rope_type, rope_theta, ...}; earlier versions rope_theta and
+  // rope_scaling {rope_type (or type), ...} (null = none).  Defaults are transformers' LlamaConfig ones.
+  const Json* rp = cfg.get("rope_parameters");
+  if (rp && !rp->is_object()) rp = nullptr;
+  const Json* rs = rp ? rp : cfg.get("rope_scaling");
+  if (rs && !rs->is_null() && !rs->is_object()) return fail("rope_scaling is not an object");
+  if (rs && rs->is_null()) rs = nullptr;
+  const double theta = num(&cfg, "rope_theta", num(rp, "rope_theta", 10000.0));
+  if (!(theta > 1.0) || !std::isfinite(theta)) return fail("rope_theta must be finite and > 1");
+  const double eps = num(&cfg, "rms_norm_eps", 1e-6);
+  if (!(eps > 0.0) || !std::isfinite(eps)) return fail("rms_norm_eps must be finite and > 0");
+  std::string type = str(rs, "rope_type");
+  if (type.empty()) type = str(rs, "type");
+  std::string e;
+  if (!rope_scaling_factors(type, num(rs, "factor", 0), num(rs, "low_freq_factor", 0), num(rs, "high_freq_factor", 0),
+                            num(rs, "original_max_position_embeddings", 0), theta, 128, &geo_.rope_freq_factors, &e))
+    return fail(e);
+  geo_.rope_theta = float(theta);
+  geo_.rms_eps = float(eps);
+  geo_.rope_scaling = geo_.rope_freq_factors.empty() ? "none" : type;
+  geo_.rope_known = true;
   return true;
 }
 
@@ -348,7 +441,11 @@ bool Checkpoint::open_gguf(std::string* err) {
   const uint64_t base = (uint64_t(c.p - data_) + alignment - 1) / alignment * alignment;
   const uint32_t n_head = u32_of(g("attention.head_count", 1)), n_kv_head = u32_of(g("attention.head_count_kv", n_head));
   bool has_output = false;
-  for (const Info& in : infos) has_output |= in.name == "output.weight";
+  const Info* rope_freqs = nullptr;   // llama.cpp's per-frequency RoPE divisors (Llama 3.1+ llama3 scaling)
+  for (const Info& in : infos) {
+    has_output |= in.name == "output.weight";
+    if (in.name == "rope_freqs.weight") rope_freqs = &in;
+  }
   for (const Info& in : infos) {
     uint32_t per = 0, bsz = 0;
     if (!block_shape(in.type, &per, &bsz)) { if (err) *err = "gguf: tensor " + in.name + " has unsupported ggml type " + std::to_string(in.type); return false; }
@@ -396,6 +493,32 @@ bool Checkpoint::open_gguf(std::string* err) {
   geo_.rope_theta = float(g("rope.freq_base", 10000.0));
   geo_.rms_eps = float(g("attention.layer_norm_rms_epsilon", 1e-5));
   geo_.known = geo_.hidden && geo_.n_layers && geo_.n_heads && geo_.ffn && geo_.vocab;
+  // RoPE scaling: the rope_freqs tensor (bit for bit) and/or {arch}.rope.scaling.type = linear with its factor
+  geo_.rope_known = true;
+  if (rope_freqs) {
+    const uint64_t want = geo_.head_dim / 2;
+    if (rope_freqs->type != kF32 || rope_freqs->dims.size() != 1 || rope_freqs->dims[0] != want || want == 0) {
+      if (err) *err = "gguf: rope_freqs.weight must be " + std::to_string(want) + " F32 values (head_dim / 2)";
+      return false;
+    }
+    geo_.rope_freq_factors.resize(size_t(want));
+    memcpy(geo_.rope_freq_factors.data(), data_ + base + rope_freqs->off, size_t(want) * 4);   // bounds checked in the loop above
+    for (float v : geo_.rope_freq_factors)
+      if (!(v > 0.f) || !std::isfinite(v)) { if (err) *err = "gguf: rope_freqs.weight holds a factor that is not finite and > 0"; return false; }
+    geo_.rope_scaling = "rope_freqs";
+  }
+  const auto st = str.find(arch + ".rope.scaling.type");
+  const std::string stype = st == str.end() ? std::string() : st->second;
+  if (!stype.empty() && stype != "none") {
+    std::vector<float> lin;
+    std::string e;
+    if (stype != "linear") e = "unsupported RoPE scaling type '" + stype + "': only linear and rope_freqs.weight are served";
+    else rope_scaling_factors(stype, g("rope.scaling.factor", 0), 0, 0, 0, 0, geo_.head_dim, &lin, &e);
+    if (!e.empty() || lin.empty()) { if (err) *err = "gguf: " + (e.empty() ? std::string("bad RoPE scaling") : e); return false; }
+    if (geo_.rope_freq_factors.empty()) geo_.rope_freq_factors = lin;
+    else for (size_t j = 0; j < lin.size(); ++j) geo_.rope_freq_factors[j] *= lin[j];   // llama.cpp applies both
+    geo_.rope_scaling = "linear";
+  }
   tok_model_ = str.count("tokenizer.ggml.model") ? str["tokenizer.ggml.model"] : "";
   tok_pre_ = str.count("tokenizer.ggml.pre") ? str["tokenizer.ggml.pre"] : "llama-bpe";
   tok_bos_ = num.count("tokenizer.ggml.bos_token_id") ? i64_of(num["tokenizer.ggml.bos_token_id"], -1) : -1;
@@ -501,6 +624,11 @@ int llmlb_ckpt_geometry(void* c, uint32_t* u7, float* f2) {
   memcpy(u7, v, sizeof v);
   f2[0] = g.rope_theta; f2[1] = g.rms_eps;
   return g.known ? 1 : 0;
+}
+uint32_t llmlb_ckpt_rope_freq_factors(void* c, float* out, uint32_t cap) {
+  const auto& f = static_cast<Checkpoint*>(c)->geometry().rope_freq_factors;
+  for (size_t j = 0; j < f.size() && j < cap && out; ++j) out[j] = f[j];
+  return uint32_t(f.size());
 }
 int64_t llmlb_ckpt_tensor_info(void* c, uint32_t i, char* name, uint32_t name_cap, uint64_t* rows, uint64_t* cols) {
   const auto& ts = static_cast<Checkpoint*>(c)->tensors();

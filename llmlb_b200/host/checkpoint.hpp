@@ -28,7 +28,21 @@ struct CkptGeometry {               // the fields of llmlb_model_config, when th
   bool known = false;
   uint32_t hidden = 0, n_layers = 0, n_heads = 0, n_kv_heads = 0, head_dim = 0, ffn = 0, vocab = 0;
   float rope_theta = 10000.f, rms_eps = 1e-5f;
+  // RoPE frequency scaling as fixed per-frequency divisors (inv_freq[j] = theta^(-2j/hd) / f[j]).
+  // rope_known: the file states theta, eps and the scaling (GGUF metadata, or a config.json beside a
+  // safetensors file); a safetensors file without one has no say.  rope_scaling: "none", "llama3",
+  // "linear" or "rope_freqs" (a GGUF per-frequency tensor); rope_freq_factors: head_dim/2 values, empty = none.
+  bool rope_known = false;
+  std::string rope_scaling = "none";
+  std::vector<float> rope_freq_factors;
 };
+
+// The divisors of a llama3 or linear `rope_scaling` (rope_type / type, factor, ...; transformers'
+// _compute_llama3_parameters / _compute_linear_scaling_rope_parameters), computed in fp64.  "default" or
+// "none" give no factors.  Any other type (dynamic, yarn, longrope: tables that depend on the sequence
+// length or scale attention) is refused: false + *err.
+bool rope_scaling_factors(const std::string& type, double factor, double low_freq_factor, double high_freq_factor,
+                          double original_ctx, double theta, uint32_t head_dim, std::vector<float>* out, std::string* err);
 
 class Checkpoint {
  public:
@@ -47,7 +61,9 @@ class Checkpoint {
 
  private:
   bool open_safetensors(std::string* err);
+  bool read_config_json(int64_t max_layer, std::string* err);   // safetensors: config.json beside the file, if any
   bool open_gguf(std::string* err);
+  std::string path_;
   const uint8_t* data_ = nullptr;
   size_t size_ = 0;
   bool gguf_ = false, tied_lm_head_ = false;

@@ -32,6 +32,10 @@
 #include <vector>
 
 #include "../../include/llmlb_b200.h"
+// Added to the ABI without a version bump: referenced weakly, so that this server still links and runs against an
+// engine library of the same ABI version that predates it (and refuses a scaled checkpoint there instead of serving it
+// unscaled), such as the scripted engine the CPU tests link it against.
+#pragma weak llmlb_engine_set_rope_freq_factors
 #include "anthropic.hpp"
 #include "checkpoint.hpp"
 #include "download.hpp"
@@ -558,6 +562,15 @@ static bool merge_geometry(CkptGeometry* g, const CkptGeometry& f, std::string* 
   };
   g->n_layers = std::max(g->n_layers, f.n_layers);
   if (f.known || f.hidden) { g->rope_theta = f.rope_theta; g->rms_eps = f.rms_eps; }
+  if (f.rope_known) {   // RoPE scaling: every file that states one must state the same
+    if (g->rope_known && (g->rope_scaling != f.rope_scaling || g->rope_freq_factors != f.rope_freq_factors ||
+                          g->rope_theta != f.rope_theta || g->rms_eps != f.rms_eps)) {
+      *err = "the weight files disagree about RoPE theta / scaling or RMSNorm eps";
+      return false;
+    }
+    g->rope_known = true; g->rope_scaling = f.rope_scaling; g->rope_freq_factors = f.rope_freq_factors;
+    g->rope_theta = f.rope_theta; g->rms_eps = f.rms_eps;
+  }
   return take(&g->hidden, f.hidden, "hidden") && take(&g->n_heads, f.n_heads, "n_heads") && take(&g->n_kv_heads, f.n_kv_heads, "n_kv_heads") &&
          take(&g->head_dim, f.head_dim, "head_dim") && take(&g->ffn, f.ffn, "ffn") && take(&g->vocab, f.vocab, "vocab");
 }
@@ -571,7 +584,7 @@ struct WeightPlan {
 // buffers that ship inside checkpoints but are not model weights
 static bool is_ignorable_tensor(const std::string& n) {
   auto ends = [&](const char* suf) { const size_t l = strlen(suf); return n.size() >= l && n.compare(n.size() - l, l, suf) == 0; };
-  return ends("rotary_emb.inv_freq") || ends("rope_freqs.weight") || ends(".attn.bias") || ends(".masked_bias");
+  return ends("rotary_emb.inv_freq") || ends(".attn.bias") || ends(".masked_bias");
 }
 
 static bool plan_weights(const llmlb_model_config& m, const std::vector<std::unique_ptr<Checkpoint>>& ckpts, WeightPlan* plan, std::string* err) {
@@ -655,16 +668,19 @@ int main(int argc, char** argv) {
   // spreads the layers over its shards), every tensor validated BEFORE the engine exists, and
   // start-up fails unless every weight of the model was found (no silently synthetic layers)
   std::vector<std::unique_ptr<Checkpoint>> ckpts;
+  CkptGeometry merged{};             // what the files say (the model with --model auto), RoPE scaling included
   for (const auto& wf : weight_files) {
     std::string err;
     ckpts.emplace_back(new Checkpoint());
     if (!ckpts.back()->open(wf, &err)) { fprintf(stderr, "weights %s: %s\n", wf.c_str(), err.c_str()); return 2; }
   }
+  {
+    std::string err;
+    for (const auto& c : ckpts) if (!merge_geometry(&merged, c->geometry(), &err)) { fprintf(stderr, "weights: %s\n", err.c_str()); return 2; }
+  }
   if (geometry == "auto") {
     if (ckpts.empty()) { fprintf(stderr, "--model auto needs --weights with a file that describes the model\n"); return 2; }
-    CkptGeometry g{};
-    std::string err;
-    for (const auto& c : ckpts) if (!merge_geometry(&g, c->geometry(), &err)) { fprintf(stderr, "weights: %s\n", err.c_str()); return 2; }
+    const CkptGeometry& g = merged;
     if (!(g.hidden && g.n_layers && g.n_heads && g.n_kv_heads && g.ffn && g.vocab)) { fprintf(stderr, "--model auto: the weight files do not describe the whole model (hidden %u, layers %u, heads %u/%u, ffn %u, vocab %u)\n", g.hidden, g.n_layers, g.n_heads, g.n_kv_heads, g.ffn, g.vocab); return 2; }
     cfg.model = {g.hidden, g.n_layers, g.n_heads, g.n_kv_heads, g.head_dim ? g.head_dim : 128, g.ffn, g.vocab, g.rope_theta, g.rms_eps};
   }
@@ -698,13 +714,29 @@ int main(int argc, char** argv) {
   }
   if (dry_run) {   // everything that does not need the GPU has been checked: report and leave
     const llmlb_model_config& m = cfg.model;
+    const auto& rf = merged.rope_freq_factors;
+    char rope[256];
+    if (rf.empty()) snprintf(rope, sizeof rope, "{\"type\":\"none\"}");
+    else snprintf(rope, sizeof rope, "{\"type\":\"%s\",\"factors\":%zu,\"min_factor\":%.9g,\"max_factor\":%.9g}", merged.rope_scaling.c_str(),
+                  rf.size(), double(*std::min_element(rf.begin(), rf.end())), double(*std::max_element(rf.begin(), rf.end())));
     printf("{\"dry_run\":true,\"model\":{\"hidden\":%u,\"n_layers\":%u,\"n_heads\":%u,\"n_kv_heads\":%u,\"head_dim\":%u,\"ffn\":%u,\"vocab\":%u},"
-           "\"tensors_to_load\":%zu,\"lm_head_tied\":%s,\"tokenizer_entries\":%u,\"stop_ids\":%zu}\n",
+           "\"tensors_to_load\":%zu,\"lm_head_tied\":%s,\"tokenizer_entries\":%u,\"stop_ids\":%zu,\"rope_theta\":%.9g,\"rope_scaling\":%s}\n",
            m.hidden, m.n_layers, m.n_heads, m.n_kv_heads, m.head_dim, m.ffn, m.vocab, plan.loads.size(), plan.lm_head_tied ? "true" : "false",
-           G.tok ? G.tok->vocab_size() : 0u, G.stop_ids.size());
+           G.tok ? G.tok->vocab_size() : 0u, G.stop_ids.size(), double(m.rope_theta), rope);
     return 0;
   }
   if (llmlb_engine_create(&cfg, &G.eng) != LLMLB_OK) { fprintf(stderr, "engine: %s\n", llmlb_last_error()); return 2; }
+  if (!merged.rope_freq_factors.empty()) {   // before the first request: the engine's RoPE table is rebuilt with the divisors
+    if (!llmlb_engine_set_rope_freq_factors) {
+      fprintf(stderr, "engine: the checkpoint needs RoPE frequency scaling (%s), which this engine library does not provide\n", merged.rope_scaling.c_str());
+      return 2;
+    }
+    if (llmlb_engine_set_rope_freq_factors(G.eng, merged.rope_freq_factors.data(), uint32_t(merged.rope_freq_factors.size())) != LLMLB_OK) {
+      fprintf(stderr, "engine: RoPE scaling: %s\n", llmlb_last_error());
+      return 2;
+    }
+    fprintf(stderr, "rope: %s scaling, %zu frequency factors\n", merged.rope_scaling.c_str(), merged.rope_freq_factors.size());
+  }
   {
     std::vector<uint16_t> bits;
     for (const WeightPlan::Load& ld : plan.loads) {
