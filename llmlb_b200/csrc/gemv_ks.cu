@@ -41,6 +41,8 @@ constexpr int kKsWarps = 16;
 static __device__ TraceBuf d_trace_ks;
 void ks_set_trace(const TraceBuf& tb) { cudaMemcpyToSymbol(d_trace_ks, &tb, sizeof(tb)); }
 
+// PTX names barriers 0..15 and __syncthreads() owns 0, so a team's id 1 + team must stay <= 15: at most 15 teams, which
+// is why ks_pick never returns TW < 2 (16 / TW <= 8 teams)
 __device__ __forceinline__ void team_barrier(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
@@ -339,14 +341,15 @@ gemv_ks_kernel(const __nv_bfloat16* __restrict__ W, const void* xin /* predecess
   }
 }
 
-// picks (TW, CW): TW*CW*256 == K, TW <= 16, CW in {1,2,4}, B*CW <= 4.  Returns false if none.
+// picks (TW, CW): TW*CW*256 == K, 2 <= TW <= 16, CW in {1,2,4}, B*CW <= 4.  Returns false if none.  TW = 1 would make
+// 16 teams, one more than there are named barriers for them (team_barrier); K = 256 goes to the row-owner kernel instead.
 static bool ks_pick(uint32_t n_tokens, uint32_t K, uint32_t* tw, uint32_t* cw) {
   if (K % 256) return false;
   const uint32_t chunks = K / 256;
   for (uint32_t c : {1u, 2u, 4u}) {
     if (chunks % c) continue;
     uint32_t t = chunks / c;
-    if (t <= 16 && n_tokens * c <= 4) { *tw = t; *cw = c; return true; }
+    if (t >= 2 && t <= 16 && n_tokens * c <= 4) { *tw = t; *cw = c; return true; }
   }
   return false;
 }

@@ -210,7 +210,8 @@ cudaError_t cudaGraphExecDestroy(cudaGraphExec_t x) { free(x); return cudaSucces
 // cluster dims and whether it was launched as a programmatic dependent (PDL) — the engine's LAUNCH PLAN for any geometry,
 // readable without a GPU (tests/test_launch_plan_cpu.py checks co-residency and resource limits on it).  Launches of the
 // projection GEMMs (gemm_tc_kernel / gemm_tc2_kernel, whose 10th parameter is split_k) append that K-split count, so that
-// tests/test_kernel_coverage_cpu.py can tell a K-split launch from a plain one.
+// tests/test_kernel_coverage_cpu.py can tell a K-split launch from a plain one.  Launches of the K-split decode GEMV
+// (gemv_ks_kernel, whose 9th parameter is TW, the warps of a team) append TW, which sets the kernel's team count.
 static void log_launch(const void* fn, dim3 g, dim3 b, size_t smem, dim3 cluster, int pdl, void** args = nullptr) {
   static FILE* f = getenv("FAKE_CUDART_LAUNCH_LOG") ? fopen(getenv("FAKE_CUDART_LAUNCH_LOG"), "a") : nullptr;
   if (!f) return;
@@ -219,6 +220,7 @@ static void log_launch(const void* fn, dim3 g, dim3 b, size_t smem, dim3 cluster
   const char* name = it == g_kernels.end() ? "?" : it->second.c_str();
   fprintf(f, "%s %u %u %u %u %u %u %zu %u %u %u %d", name, g.x, g.y, g.z, b.x, b.y, b.z, smem, cluster.x, cluster.y, cluster.z, pdl);
   if (args && (strstr(name, "gemm_tc_kernel") || strstr(name, "gemm_tc2_kernel"))) fprintf(f, " %u", *static_cast<const uint32_t*>(args[9]));
+  if (args && strstr(name, "gemv_ks_kernel")) fprintf(f, " %u", *static_cast<const uint32_t*>(args[8]));
   fputc('\n', f);
   fflush(f);
 }

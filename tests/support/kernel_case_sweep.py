@@ -1,8 +1,10 @@
-"""The launches of the GPU kernel tests (tests/test_kernels_sm90_gpu.py), made over the fake CUDA runtime with
-FAKE_CUDART_LAUNCH_LOG set: every GEMM case through the entry point it uses there, the wave-tail pair, every decode split and
-both prefill attention kernels.  Nothing executes; the log is the launch plan of the test cases.
+"""The launches of the GPU kernel tests (tests/test_kernels_sm90_gpu.py, tests/test_gemv_sm90_gpu.py), made over the fake
+CUDA runtime with FAKE_CUDART_LAUNCH_LOG set: every GEMM case through the entry point it uses there, the wave-tail pair, every
+decode split, both prefill attention kernels and every GEMV case through llmlb_op_gemv.  Nothing executes; the log is the
+launch plan of the test cases.  Every section is optional.
 usage: kernel_case_sweep.py <cases.json>   ({"gemm": [[T, n_out, K, epi], ...], "wave_tail": [T, n_out, K, main_rows],
-                                             "decode_splits": [...], "max_split": n})"""
+                                             "decode_splits": [...], "max_split": n,
+                                             "gemv": [[n_out, K, tokens, epi, norm, out_stride], ...]})"""
 import ctypes
 import json
 import os
@@ -32,23 +34,29 @@ def mark(s):
 cases = json.load(open(sys.argv[1]))
 w, x, out = dmalloc(1 << 33), dmalloc(1 << 30), dmalloc(1 << 31)          # address space only: nothing is executed
 parts = ctypes.c_uint32()
-for T, n_out, k, epi in cases["gemm"]:
+for T, n_out, k, epi in cases.get("gemm", []):
     mark("gemm %d %d %d %d" % (T, n_out, k, epi))
     n_cols = n_out // 2 if epi == 2 else n_out
     if epi == 4:
         ffi.check(L.llmlb_debug_gemm(w, x, out, T, n_out, k, epi, n_cols, 0, 0, cases["max_split"], ctypes.byref(parts), None))
     else:
         ffi.check(L.llmlb_op_gemm(w, x, out, T, n_out, k, epi, n_cols, 0, None))
-T, n_out, k, rows = cases["wave_tail"]
-for epi in (2, 3):
-    mark("wave tail %d" % epi)
-    n_cols = n_out // 2 if epi == 2 else n_out
-    for row0, n_rows in ((0, 0), (0, rows), (rows, n_out - rows)):
-        ffi.check(L.llmlb_debug_gemm(w, x, out, T, n_out, k, epi, n_cols, row0, n_rows, cases["max_split"], ctypes.byref(parts), None))
+if "wave_tail" in cases:
+    T, n_out, k, rows = cases["wave_tail"]
+    for epi in (2, 3):
+        mark("wave tail %d" % epi)
+        n_cols = n_out // 2 if epi == 2 else n_out
+        for row0, n_rows in ((0, 0), (0, rows), (rows, n_out - rows)):
+            ffi.check(L.llmlb_debug_gemm(w, x, out, T, n_out, k, epi, n_cols, row0, n_rows, cases["max_split"], ctypes.byref(parts), None))
 rope, ws = dmalloc(1 << 20), dmalloc(256)
-for sp in cases["decode_splits"]:
+for sp in cases.get("decode_splits", []):
     mark("decode %d" % sp)
     ffi.check(L.llmlb_op_decode_attention(x, w, w, out, 66, out, out, 5, out, 32, 8, rope, sp, 5, ws, None))
-mark("prefill")
-ffi.check(L.llmlb_op_prefill_attention_tc(x, 300, w, w, 80, out, 66, out, 3, out, 32, 8, None))
-ffi.check(L.llmlb_op_prefill_attention(x, w, w, out, 66, out, 3, out, 32, 8, None))
+if "decode_splits" in cases:
+    mark("prefill")
+    ffi.check(L.llmlb_op_prefill_attention_tc(x, 300, w, w, 80, out, 66, out, 3, out, 32, 8, None))
+    ffi.check(L.llmlb_op_prefill_attention(x, w, w, out, 66, out, 3, out, 32, 8, None))
+gain = dmalloc(1 << 20)
+for n_out, k, n_tok, epi, norm, out_stride in cases.get("gemv", []):
+    mark("gemv %d %d %d %d %d" % (n_out, k, n_tok, epi, norm))
+    ffi.check(L.llmlb_op_gemv(w, x, gain if norm else None, 1e-5, out, n_tok, n_out, k, epi, out_stride, None))

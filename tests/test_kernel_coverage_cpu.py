@@ -10,6 +10,11 @@ would notice the mistakes they are meant to catch.
   * teeth: the probe comparison and the attention bound, applied with torch on the CPU to outputs that are wrong in the ways
     a kernel goes wrong (swapped 8-row groups, a dropped k16 step, swapped token halves, a causal mask off by one, a dropped
     64-token page, a running sum l that is not rescaled), must reject every one of them.
+  * decode GEMVs (tests/test_gemv_sm90_gpu.py): the GEMV cases launch every GEMV class — K-split kernel (B, epilogue, NORM,
+    CW, TW) or row-owner kernel (B, epilogue, NORM) — that the tp = 1 engine launches at Llama-3-8B, LLAMA_MID and
+    Llama-3-70B shapes (prefill widths and decode batches 1..4: wider steps use the GEMMs); every K-split launch for
+    K = 256 j, j = 1..400, and 1..4 tokens has at most 15 teams, so its named barriers 1 + team stay within PTX's 0..15;
+    and the GEMV probe and bounds reject outputs wrong in the ways these kernels go wrong.
 """
 import collections
 import json
@@ -25,14 +30,18 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 import test_engine_host_logic_cpu as HL  # noqa: E402
+import test_gemv_sm90_gpu as GV  # noqa: E402
 import test_kernels_sm90_gpu as K  # noqa: E402
 
 GEMM_RE = re.compile(r"(gemm_tc2?_kernel)ILi(\d+)ELi(\d+)E")
+GEMV_KS_RE = re.compile(r"14gemv_ks_kernelILi(\d+)ELi(\d+)ELb([01])ELi(\d+)ELi(\d+)E")
+GEMV_RE = re.compile(r"11gemv_kernelILi(\d+)ELi(\d+)ELb([01])E")
 
 
 def classes(log):
     """{context: set of launch classes}: ("gemm_tc_kernel" | "gemm_tc2_kernel", BN, EPI, K-split) for the projections,
-    ("decode", cluster size) for decode attention (1 = the unsplit tensor-core kernel), ("prefill", kernel)."""
+    ("decode", cluster size) for decode attention (1 = the unsplit tensor-core kernel), ("prefill", kernel),
+    ("gemv_ks", B, EPI, NORM, CW, TW) for the K-split GEMV and ("gemv", B, EPI, NORM) for the row-owner GEMV."""
     out, ctx = collections.defaultdict(set), "init"
     for line in open(log):
         if line.startswith("###"):
@@ -43,6 +52,15 @@ def classes(log):
         if m:
             assert len(p) == 13, line            # the fake runtime appends split_k to projection launches
             out[ctx].add((m.group(1), int(m.group(2)), int(m.group(3)), int(p[12]) > 1))
+            continue
+        m = GEMV_KS_RE.search(p[0])
+        if m:
+            assert len(p) == 13 and m.group(5) == "0", line     # TW appended; no tensor-parallel variant at tp = 1
+            out[ctx].add(("gemv_ks", int(m.group(1)), int(m.group(2)), m.group(3) == "1", int(m.group(4)), int(p[12])))
+            continue
+        m = GEMV_RE.search(p[0])
+        if m:
+            out[ctx].add(("gemv", int(m.group(1)), int(m.group(2)), m.group(3) == "1"))
         elif "decode_attention_mma_kernel" in p[0]:
             out[ctx].add(("decode", 1))
         elif "decode_attention_kernel" in p[0]:
@@ -208,3 +226,237 @@ def test_attention_bound_rejects_a_dropped_page(scale):
 def test_attention_bound_rejects_an_unrescaled_running_sum(scale):
     q, k, v, kp, vp, pos = _attn_case(scale)
     assert _over_bound(_online(q, kp, vp, pos, lambda s, p: s <= p, rescale_l=False), q, k, v, pos) > 0
+
+
+# ------------------------------------------------------------------------------------------------------ decode GEMVs --
+EPIS = (K.EPI_STORE_BF16, K.EPI_RESID_F32, K.EPI_SILU_MUL, K.EPI_STORE_F32)
+KS_INSTANCES = ((1, 1), (1, 2), (1, 4), (2, 1), (2, 2), (3, 1), (4, 1))    # (B, CW) of gemv_ks_try's dispatch
+
+
+def _gemv_sweep(tmp_path, name, rows):
+    """The classes of llmlb_op_gemv launches over the fake runtime, per case: rows of (n_out, K, tokens, epi, norm)."""
+    spec = tmp_path / (name + ".json")
+    spec.write_text(json.dumps({"gemv": [[N, Kd, B, e, int(n), GV.n_cols(N, e) + GV.PAD] for N, Kd, B, e, n in rows]}))
+    return run_logged(tmp_path, name, [os.path.join(HERE, "support", "kernel_case_sweep.py"), str(spec)])
+
+
+def _gemv_classes(per_ctx):
+    return {c for cs in per_ctx.values() for c in cs if c[0] in ("gemv_ks", "gemv")}
+
+
+def test_gpu_gemv_cases_launch_every_gemv_class_the_engine_launches(built_lib, tmp_path):
+    per_case = _gemv_sweep(tmp_path, "gemv_cases", GV.gemv_params())
+    tested = _gemv_classes(per_case)
+    engine = {}
+    for model in ("8b", "mid", "70b"):
+        plan = run_logged(tmp_path, "engine_" + model, [os.path.join(HERE, "support", "launch_plan_sweep.py"), model, "1", "4"])
+        for c in _gemv_classes(plan):
+            engine.setdefault(c, model)
+    assert len(engine) >= 40 and {c[0] for c in engine} == {"gemv_ks", "gemv"}, sorted(engine)
+    missing = sorted((c, model) for c, model in engine.items() if c not in tested)
+    assert not missing, "the engine launches GEMV classes no GPU GEMV test runs (class, model): %s" % missing
+    # what the case table promises besides: every K-split instantiation with every epilogue, with and without NORM; the
+    # team shapes TW 16, 14, 8, 7, 3, 2 (CW 1), 14 and 16 (CW 2), 14 (CW 4); every row-owner instantiation
+    ks = {c for c in tested if c[0] == "gemv_ks"}
+    missing = sorted({(B, cw, e, n) for B, cw in KS_INSTANCES for e in EPIS for n in (False, True)} - {(c[1], c[4], c[2], c[3]) for c in ks})
+    assert not missing, "no GPU GEMV case launches the K-split instantiations (B, CW, EPI, NORM) %s" % missing
+    missing = sorted({(1, 16), (1, 14), (1, 8), (1, 7), (1, 3), (1, 2), (2, 14), (2, 16), (4, 14)} - {(c[4], c[5]) for c in ks})
+    assert not missing, "no GPU GEMV case launches the K-split team shapes (CW, TW) %s" % missing
+    missing = sorted({("gemv", B, e, n) for B in (1, 2, 3, 4) for e in EPIS for n in (False, True)} - tested)
+    assert not missing, "no GPU GEMV case launches the row-owner instantiations %s" % missing
+    assert per_case["gemv 8454 28672 4 1 0"] == {("gemv", 1, K.EPI_RESID_F32, False)}      # one row-owner pass per token
+    assert per_case["gemv 264 256 1 3 0"] == {("gemv", 1, K.EPI_STORE_F32, False)}          # K = 256: no one-warp teams
+
+
+def test_every_k_split_gemv_launch_keeps_its_team_barriers_in_range(built_lib, tmp_path):
+    """gemv_ks_kernel synchronises team t with named barrier 1 + t and runs 16 // TW teams; PTX has barriers 0..15."""
+    per_case = _gemv_sweep(tmp_path, "gemv_barriers", [(8, 256 * j, B, K.EPI_STORE_F32, False)
+                                                       for j in range(1, 401) for B in (1, 2, 3, 4)])
+    n_ks = 0
+    for ctx, cs in per_case.items():
+        for c in cs:
+            if c[0] == "gemv_ks":
+                n_ks += 1
+                assert 16 // c[5] <= 15, "%s: TW %d makes %d teams, barrier ids up to %d" % (ctx, c[5], 16 // c[5], 16 // c[5])
+    assert n_ks >= 60, n_ks                     # K = 512 .. 16384 where ks_pick finds a team shape
+
+
+# GEMV teeth: a model GEMV on the CPU, right or wrong in one of the ways these kernels go wrong, checked by the GPU test's
+# probe and bounds.  Case: K = 2048 (8 chunks of 256: a K-split team of 8 warps), 264 rows, 2 tokens.
+TN, TK, TB = 264, 2048, 2
+
+
+def _model(w, x, epi, prev=None, gain=None, eps=0.0, gain_shift=0, rs_from=None, gate_up=None, resid=None):
+    """epi(W . y) in fp64 with the kernels' rounding points: y = x (bf16), or y = bf16(x rs g) with NORM."""
+    y = x.double()
+    if gain is not None:
+        rs = (y.pow(2).mean(-1, keepdim=True) + eps).rsqrt()
+        if rs_from is not None:
+            rs = rs[rs_from]
+        y = (y * rs * gain.double().roll(-gain_shift)).to(torch.bfloat16).double()
+    acc = (y @ w.double().t()).float()
+    if epi == K.EPI_SILU_MUL:
+        g, u = acc[:, 0::2].double(), acc[:, 1::2].double()
+        if gate_up:
+            g, u = gate_up(g, u)
+        return (g / (1 + (-g).exp()) * u).to(torch.bfloat16)
+    if epi == K.EPI_RESID_F32:
+        return resid(prev, acc) if resid else prev + acc
+    return acc.to(torch.bfloat16) if epi == K.EPI_STORE_BF16 else acc
+
+
+def _probe_rejects(epi=K.EPI_STORE_F32, norm=False, mutate_x=None, **knobs):
+    """Mismatches the GEMV probe finds over all rounds of the teeth case."""
+    w = K.probe_weights(TN, TK, torch.Generator().manual_seed(5), "cpu")
+    plan = GV.probe_plan(TB, TK, norm, 11)
+    e, gain, eps = GV.probe_norm_setup(TK, plan[0][0].shape[1], 11, "cpu") if norm else (None, None, 0.0)
+    prev = K.probe_weights(TB, GV.n_cols(TN, epi), torch.Generator().manual_seed(6), "cpu").float()
+    bad = 0
+    for cols, signs in plan:
+        x, acc = GV.probe_x_and_ref(w, cols, signs, e)
+        out = _model(w, mutate_x(x.clone()) if mutate_x else x, epi, prev, gain, eps, **knobs)
+        bad += GV.probe_mismatches(out, acc, epi, prev)
+    return bad
+
+
+def _random_rejects(epi=K.EPI_STORE_F32, norm=False, B=TB, **knobs):
+    """Elements over the GEMV random-data bound."""
+    w = GV.random_w(TN, TK, 3, "cpu")
+    x, gain = GV.random_x(B, TK, norm, 4, "cpu")
+    prev = torch.randn(B, TN, generator=torch.Generator().manual_seed(7))
+    out = _model(w, x, epi, prev, gain if norm else None, GV.RANDOM_EPS, **knobs)
+    ref, bound, _ = GV.random_ref(w, x, epi, prev, gain if norm else None, GV.RANDOM_EPS)
+    return GV.over_bound(out, ref, bound)[0]
+
+
+def test_gemv_case_table_probe_covers_every_8_group_of_every_token():
+    for _, Kd, toks, _, norms in GV.GEMV_CASES:
+        for B in toks:
+            for norm in norms:
+                plan = GV.probe_plan(B, Kd, norm, 1)
+                for t in range(B):
+                    hit = torch.cat([cols[t] for cols, _ in plan])
+                    assert set((hit // 8).tolist()) == set(range(Kd // 8)), (Kd, B, norm, t)
+                    assert len(set((hit % 8).tolist())) == min(8, len(hit)), (Kd, B, norm, t)
+                assert all(len(set((cols[t] // 8).tolist())) == cols.shape[1] for cols, _ in plan for t in range(B))
+
+
+@pytest.mark.parametrize("norm", [False, True])
+@pytest.mark.parametrize("epi", EPIS)
+def test_gemv_probe_and_bound_accept_a_correct_gemv(epi, norm):
+    assert _probe_rejects(epi, norm) == 0
+    assert _random_rejects(epi, norm) == 0
+    assert _random_rejects(epi, norm, B=4) == 0
+
+
+@pytest.mark.parametrize("norm", [False, True])
+def test_gemv_probe_rejects_a_dropped_or_neighbouring_256_chunk(norm):
+    for j in range(TK // 256):
+        lo, hi = 256 * j, 256 * j + 256
+
+        def drop(x):
+            x[:, lo:hi] = 0
+            return x
+
+        def neighbour(x):                   # the warp reads W and x at the next warp's offset: chunk j + 1 twice, j never
+            x[:, lo:hi], x[:, hi % TK:hi % TK + 256] = 0, 2 * x[:, hi % TK:hi % TK + 256]
+            return x
+        assert _probe_rejects(norm=norm, mutate_x=drop) > 0, j
+        assert _probe_rejects(norm=norm, mutate_x=neighbour) > 0, j
+
+
+@pytest.mark.parametrize("norm", [False, True])
+def test_gemv_probe_rejects_a_shifted_8_group(norm):
+    for g in (0, 1, 31, 32, 33, 100, 255):
+        def shift(x, g=g):                  # the lane's activations come from the next 8-group (its weights do not)
+            nxt = (g + 1) % (TK // 8)
+            x[:, 8 * g:8 * g + 8] = x[:, 8 * nxt:8 * nxt + 8].clone()
+            return x
+        assert _probe_rejects(norm=norm, mutate_x=shift) > 0, g
+
+
+RN = 266       # 133 row pairs over gemv_ks's 132 CTAs: CTA ranges of one and of two pairs
+
+
+def _ks_rows(b, grid, n_pairs, n_out):
+    """gemv_ks_kernel's rows of CTA b: whole row pairs, in contiguous near-equal ranges."""
+    return (b * n_pairs // grid) * 2, min(n_out, ((b + 1) * n_pairs // grid) * 2)
+
+
+def _ranged_output(acc, epi, prev, rows_of):
+    """What the CTAs of a gemv_ks launch write when CTA b takes rows rows_of(b, grid, n_pairs, n_out): each CTA applies the
+    epilogue to its own rows (SiLU to the pairs (r, r + 1) counted from its first row while r + 1 is in range; the
+    residual add accumulates, so a row two CTAs take gets it twice); rows no CTA takes keep the NaN sentinel."""
+    n_out = acc.shape[1]
+    n_pairs = (n_out + 1) // 2
+    grid = min(n_pairs, 132)                             # ks_launch
+    if epi == K.EPI_RESID_F32:
+        out = prev.clone()
+    else:
+        out = torch.full((acc.shape[0], GV.n_cols(n_out, epi)), float("nan"),
+                         dtype=torch.float32 if epi == K.EPI_STORE_F32 else torch.bfloat16)
+    for b in range(grid):
+        lo, hi = rows_of(b, grid, n_pairs, n_out)
+        if epi == K.EPI_SILU_MUL:
+            r = torch.arange(lo, max(lo, hi - 1), 2)
+            g, u = acc[:, r].double(), acc[:, r + 1].double()
+            out[:, r >> 1] = (g / (1 + (-g).exp()) * u).to(torch.bfloat16)
+        elif epi == K.EPI_RESID_F32:
+            out[:, lo:hi] += acc[:, lo:hi]
+        else:
+            out[:, lo:hi] = acc[:, lo:hi].to(out.dtype)
+    return out
+
+
+def _range_rejects(epi, rows_of):
+    w = K.probe_weights(RN, 512, torch.Generator().manual_seed(8), "cpu")
+    prev = K.probe_weights(TB, RN, torch.Generator().manual_seed(9), "cpu").float()
+    bad = 0
+    for cols, signs in GV.probe_plan(TB, 512, False, 12):
+        _, acc = GV.probe_x_and_ref(w, cols, signs)
+        bad += GV.probe_mismatches(_ranged_output(acc, epi, prev, rows_of), acc, epi, prev)
+    return bad
+
+
+def test_gemv_ks_cta_ranges_are_uneven_at_266_rows():
+    lens = {hi - lo for lo, hi in (_ks_rows(b, 132, RN // 2, RN) for b in range(132))}
+    assert lens == {2, 4}
+
+
+@pytest.mark.parametrize("epi", EPIS)
+def test_gemv_probe_rejects_cta_row_ranges_that_lose_or_duplicate_a_row_pair(epi):
+    assert _range_rejects(epi, _ks_rows) == 0
+    # each range one pair short: the pair at every CTA boundary is lost
+    assert _range_rejects(epi, lambda *a: (_ks_rows(*a)[0], _ks_rows(*a)[1] - 2)) > 0
+    # each range one pair long: the pair at every boundary is computed by two CTAs, the same value twice, which only the
+    # residual add turns into a wrong result
+    long = _range_rejects(epi, lambda *a: (_ks_rows(*a)[0], min(a[3], _ks_rows(*a)[1] + 2)))
+    assert (long > 0) == (epi == K.EPI_RESID_F32)
+    # ranges cut at rows rather than pairs: harmless for rowwise epilogues, but a (gate, up) pair straddles two CTAs
+    rows = _range_rejects(epi, lambda b, grid, n_pairs, n_out: (b * n_out // grid, (b + 1) * n_out // grid))
+    assert (rows > 0) == (epi == K.EPI_SILU_MUL)
+
+
+@pytest.mark.parametrize("norm", [False, True])
+def test_gemv_probe_rejects_swapped_gate_and_up_or_the_next_pairs_up(norm):
+    assert _probe_rejects(K.EPI_SILU_MUL, norm, gate_up=lambda g, u: (u, g)) > 0
+    assert _probe_rejects(K.EPI_SILU_MUL, norm, gate_up=lambda g, u: (g, u.roll(-1, 1))) > 0
+
+
+@pytest.mark.parametrize("norm", [False, True])
+def test_gemv_probe_and_bound_reject_a_residual_added_twice(norm):
+    for resid in (lambda p, a: p + a + a, lambda p, a: p + p + a):
+        assert _probe_rejects(K.EPI_RESID_F32, norm, resid=resid) > 0
+        assert _random_rejects(K.EPI_RESID_F32, norm, resid=resid) > 0
+
+
+@pytest.mark.parametrize("epi", EPIS)
+def test_gemv_bound_rejects_another_tokens_rms_scale(epi):
+    assert _random_rejects(epi, True, rs_from=[1, 0]) > 0
+    assert _random_rejects(epi, True, B=4, rs_from=[0, 1, 2, 1]) > 0
+
+
+@pytest.mark.parametrize("epi", EPIS)
+def test_gemv_probe_rejects_a_gain_shifted_by_8(epi):
+    assert _probe_rejects(epi, True, gain_shift=8) > 0
+    assert _probe_rejects(epi, True, gain_shift=-8) > 0
