@@ -242,6 +242,13 @@ int llmlb_op_gemm(const void* w_bf16, const void* x_bf16, void* out, uint32_t n_
 int llmlb_debug_gemm(const void* w_bf16, const void* x_bf16, void* out, uint32_t n_tokens, uint32_t n_out, uint32_t k,
                      uint32_t epilogue, uint32_t out_stride, uint32_t row0, uint32_t n_rows, uint32_t max_split,
                      uint32_t* n_parts, void* stream);
+/* The residual fold between projections, as the engine launches it for steps of more than 4 tokens, for kernel tests:
+ * x[t,:] += parts[0][t,:] + ... + parts[n_parts-1][t,:] (fp32, ascending part order; part p at parts + p*part_stride
+ * floats), then, when gain != NULL, y = RMSNorm(x) * gain (bf16).  n_tokens picks the kernel as in the engine.
+ * hidden % 4 == 0, n_parts <= 16, part_stride >= n_tokens * hidden. */
+int llmlb_debug_rmsnorm_parts(float* x_f32, const float* parts_f32, uint32_t n_parts, uint64_t part_stride,
+                              const void* gain_bf16, void* y_bf16, uint32_t n_tokens, uint32_t hidden, float eps,
+                              void* stream);
 
 /* RoPE table: fp32 (cos, sin) pairs [max_pos][64] for head_dim 128, HF rotate-half pairing. */
 int llmlb_op_rope_table(float* table, uint32_t max_pos, float theta, void* stream);

@@ -112,6 +112,9 @@ __global__ void __launch_bounds__(256) rmsnorm_parts_cluster_kernel(float* __res
   __shared__ float red[8];
   __shared__ float s_ss[4];   // partial sums of squares of the 4 CTAs of the cluster (every CTA gets all four)
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  // A CTA may touch a peer's shared memory only once every CTA of the cluster is running: arrive now, wait before the
+  // first remote store (after the fold loop, so the wait costs nothing there).  Fold-only launches touch no peer.
+  if (gain) asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory");
   uint32_t cr;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(cr));
   const uint32_t t = blockIdx.x >> 2;
@@ -131,6 +134,7 @@ __global__ void __launch_bounds__(256) rmsnorm_parts_cluster_kernel(float* __res
   ss = warp_sum(ss);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = ss;
   __syncthreads();
+  asm volatile("barrier.cluster.wait.aligned;" ::: "memory");   // every peer CTA has started: its s_ss is live
   if (threadIdx.x < 4) {   // thread q stores this CTA's partial into CTA q's s_ss[cr]
     float tot = 0.f;
 #pragma unroll
@@ -224,6 +228,19 @@ extern "C" int llmlb_op_rmsnorm(const float* x, const void* gain, void* y, uint3
       x, (const __nv_bfloat16*)gain, (__nv_bfloat16*)y, hidden, eps);
   LLMLB_LAUNCH_CHECK();
   return LLMLB_OK;
+}
+
+// The residual fold + RMSNorm exactly as forward_tokens launches it between projections (kernel tests): n_tokens picks
+// the 4-CTA cluster kernel or the one-CTA-per-row kernel, as in the engine.
+extern "C" int llmlb_debug_rmsnorm_parts(float* x, const float* parts, uint32_t n_parts, uint64_t part_stride,
+                                         const void* gain, void* y, uint32_t n_tokens, uint32_t hidden, float eps,
+                                         void* stream) {
+  if (!x || (n_parts > 0 && !parts) || (gain && !y) || hidden % 4 || n_parts > 16 ||
+      part_stride < uint64_t(n_tokens) * hidden) {
+    set_error("llmlb_debug_rmsnorm_parts: bad argument");
+    return LLMLB_E_INVALID_ARG;
+  }
+  return rmsnorm_parts_launch(x, parts, n_parts, part_stride, gain, y, n_tokens, hidden, eps, (cudaStream_t)stream);
 }
 
 extern "C" int llmlb_op_synth_bf16(void* out, uint64_t rows, uint64_t cols, uint64_t row0,

@@ -91,6 +91,7 @@ PROTOTYPES = {
     "llmlb_op_gemv": (C.c_int, [vp, vp, vp, f32, vp, u32, u32, u32, u32, u32, vp]),
     "llmlb_op_gemm": (C.c_int, [vp, vp, vp, u32, u32, u32, u32, u32, u32, vp]),
     "llmlb_debug_gemm": (C.c_int, [vp, vp, vp, u32, u32, u32, u32, u32, u32, u32, u32, _P(u32), vp]),
+    "llmlb_debug_rmsnorm_parts": (C.c_int, [vp, vp, u32, u64, vp, vp, u32, u32, f32, vp]),
     "llmlb_op_rope_table": (C.c_int, [vp, u32, f32, vp]),
     "llmlb_op_rope_table_scaled": (C.c_int, [vp, u32, f32, _P(f32), vp]),
     "llmlb_op_rope_append": (C.c_int, [vp, vp, vp, vp, vp, vp, u32, u32, u32, vp]),

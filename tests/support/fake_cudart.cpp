@@ -211,24 +211,31 @@ cudaError_t cudaGraphExecDestroy(cudaGraphExec_t x) { free(x); return cudaSucces
 // readable without a GPU (tests/test_launch_plan_cpu.py checks co-residency and resource limits on it).  Launches of the
 // projection GEMMs (gemm_tc_kernel / gemm_tc2_kernel, whose 10th parameter is split_k) append that K-split count, so that
 // tests/test_kernel_coverage_cpu.py can tell a K-split launch from a plain one.  Launches of the K-split decode GEMV
-// (gemv_ks_kernel, whose 9th parameter is TW, the warps of a team) append TW, which sets the kernel's team count.
+// (gemv_ks_kernel, whose 9th parameter is TW, the warps of a team) append TW, which sets the kernel's team count.  The
+// residual fold (rmsnorm_parts_kernel / rmsnorm_parts_cluster_kernel) appends n_parts, whether a gain was given (0 / 1)
+// and hidden; rope_append_kernel appends n_heads and n_kv; rmsnorm_kernel and embed_kernel append hidden.
 static void log_launch(const void* fn, dim3 g, dim3 b, size_t smem, dim3 cluster, int pdl, void** args = nullptr) {
   static FILE* f = getenv("FAKE_CUDART_LAUNCH_LOG") ? fopen(getenv("FAKE_CUDART_LAUNCH_LOG"), "a") : nullptr;
   if (!f) return;
   std::lock_guard<std::mutex> lk(g_mu);
   auto it = g_kernels.find(fn);
   const char* name = it == g_kernels.end() ? "?" : it->second.c_str();
+  auto u32 = [&](int i) { return *static_cast<const uint32_t*>(args[i]); };
   fprintf(f, "%s %u %u %u %u %u %u %zu %u %u %u %d", name, g.x, g.y, g.z, b.x, b.y, b.z, smem, cluster.x, cluster.y, cluster.z, pdl);
-  if (args && (strstr(name, "gemm_tc_kernel") || strstr(name, "gemm_tc2_kernel"))) fprintf(f, " %u", *static_cast<const uint32_t*>(args[9]));
-  if (args && strstr(name, "gemv_ks_kernel")) fprintf(f, " %u", *static_cast<const uint32_t*>(args[8]));
+  if (args && (strstr(name, "gemm_tc_kernel") || strstr(name, "gemm_tc2_kernel"))) fprintf(f, " %u", u32(9));
+  if (args && strstr(name, "gemv_ks_kernel")) fprintf(f, " %u", u32(8));
+  if (args && strstr(name, "rmsnorm_parts"))     // (x, parts, n_parts, part_stride, gain, y, hidden, ...)
+    fprintf(f, " %u %d %u", u32(2), *static_cast<void* const*>(args[4]) != nullptr, u32(6));
+  if (args && strstr(name, "18rope_append_kernel")) fprintf(f, " %u %u", u32(6), u32(7));
+  if (args && (strstr(name, "14rmsnorm_kernel") || strstr(name, "12embed_kernel"))) fprintf(f, " %u", u32(3));
   fputc('\n', f);
   fflush(f);
 }
-cudaError_t cudaLaunchKernel(const void* fn, dim3 g, dim3 b, void**, size_t smem, cudaStream_t) {
+cudaError_t cudaLaunchKernel(const void* fn, dim3 g, dim3 b, void** args, size_t smem, cudaStream_t) {
   if (!config_allowed(g, b)) return g_last_error = cudaErrorInvalidConfiguration;
   if (!smem_allowed(fn, smem)) return g_last_error = cudaErrorInvalidValue;
   ++g_launches;
-  log_launch(fn, g, b, smem, dim3(1, 1, 1), 0);
+  log_launch(fn, g, b, smem, dim3(1, 1, 1), 0, args);
   return cudaSuccess;
 }
 cudaError_t cudaLaunchKernelExC(const cudaLaunchConfig_t* c, const void* fn, void** args) {

@@ -1,10 +1,13 @@
-"""The launches of the GPU kernel tests (tests/test_kernels_sm90_gpu.py, tests/test_gemv_sm90_gpu.py), made over the fake
-CUDA runtime with FAKE_CUDART_LAUNCH_LOG set: every GEMM case through the entry point it uses there, the wave-tail pair, every
-decode split, both prefill attention kernels and every GEMV case through llmlb_op_gemv.  Nothing executes; the log is the
-launch plan of the test cases.  Every section is optional.
+"""The launches of the GPU kernel tests (tests/test_kernels_sm90_gpu.py, tests/test_gemv_sm90_gpu.py,
+tests/test_step_kernels_sm90_gpu.py), made over the fake CUDA runtime with FAKE_CUDART_LAUNCH_LOG set: every GEMM case through
+the entry point it uses there, the wave-tail pair, every decode split, both prefill attention kernels, every GEMV case through
+llmlb_op_gemv, and the residual fold, RMSNorm, RoPE / KV-append and embedding cases.  Nothing executes; the log is the launch
+plan of the test cases.  Every section is optional.
 usage: kernel_case_sweep.py <cases.json>   ({"gemm": [[T, n_out, K, epi], ...], "wave_tail": [T, n_out, K, main_rows],
                                              "decode_splits": [...], "max_split": n,
-                                             "gemv": [[n_out, K, tokens, epi, norm, out_stride], ...]})"""
+                                             "gemv": [[n_out, K, tokens, epi, norm, out_stride], ...],
+                                             "fold": [[T, H, n_parts, gain, part_stride], ...], "rmsnorm": [[T, H], ...],
+                                             "rope": [[T, n_heads, n_kv], ...], "embed": [[T, H, vocab], ...]})"""
 import ctypes
 import json
 import os
@@ -60,3 +63,15 @@ gain = dmalloc(1 << 20)
 for n_out, k, n_tok, epi, norm, out_stride in cases.get("gemv", []):
     mark("gemv %d %d %d %d %d" % (n_out, k, n_tok, epi, norm))
     ffi.check(L.llmlb_op_gemv(w, x, gain if norm else None, 1e-5, out, n_tok, n_out, k, epi, out_stride, None))
+for T, H, n_parts, g, stride in cases.get("fold", []):
+    mark("fold %d %d %d %d %d" % (T, H, n_parts, g, stride))
+    ffi.check(L.llmlb_debug_rmsnorm_parts(out, w, n_parts, stride, gain if g else None, x if g else None, T, H, 1e-5, None))
+for T, H in cases.get("rmsnorm", []):
+    mark("rmsnorm %d %d" % (T, H))
+    ffi.check(L.llmlb_op_rmsnorm(out, gain, x, T, H, 1e-5, None))
+for T, nh, nkv in cases.get("rope", []):
+    mark("rope %d %d %d" % (T, nh, nkv))
+    ffi.check(L.llmlb_op_rope_append(x, out, out, rope, w, w, T, nh, nkv, None))
+for T, H, V in cases.get("embed", []):
+    mark("embed %d %d" % (T, H))
+    ffi.check(L.llmlb_op_embed(w, x, out, T, H, V, None))

@@ -15,6 +15,12 @@ would notice the mistakes they are meant to catch.
     Llama-3-70B shapes (prefill widths and decode batches 1..4: wider steps use the GEMMs); every K-split launch for
     K = 256 j, j = 1..400, and 1..4 tokens has at most 15 teams, so its named barriers 1 + team stay within PTX's 0..15;
     and the GEMV probe and bounds reject outputs wrong in the ways these kernels go wrong.
+  * wide-step kernels (tests/test_step_kernels_sm90_gpu.py): the cases launch every class of the residual fold (kernel,
+    n_parts, gain, H), RoPE (n_heads, n_kv, tensor-parallel shards included), final RMSNorm (H) and embedding (H) that the
+    tp = 1 engine launches at Llama-3-8B, LLAMA_MID and Llama-3-70B shapes; every kernel in those launch plans is either
+    launched by a GPU kernel test case or listed with the test that covers it; and the fold, norm and RoPE checkers reject
+    a dropped or reordered part, a gain a quarter off, a missing DSMEM exchange, another token's RMS scale, wrong RoPE
+    pairs, positions or sin sign, and K in the neighbouring page slot.
 """
 import collections
 import json
@@ -32,22 +38,48 @@ sys.path.insert(0, HERE)
 import test_engine_host_logic_cpu as HL  # noqa: E402
 import test_gemv_sm90_gpu as GV  # noqa: E402
 import test_kernels_sm90_gpu as K  # noqa: E402
+import test_step_kernels_sm90_gpu as SK  # noqa: E402
 
 GEMM_RE = re.compile(r"(gemm_tc2?_kernel)ILi(\d+)ELi(\d+)E")
 GEMV_KS_RE = re.compile(r"14gemv_ks_kernelILi(\d+)ELi(\d+)ELb([01])ELi(\d+)ELi(\d+)E")
 GEMV_RE = re.compile(r"11gemv_kernelILi(\d+)ELi(\d+)ELb([01])E")
 
 
+def short_name(mangled):
+    """The kernel's own name out of its mangled name: _ZN5llmlb14gemm_tc_kernelILi... -> gemm_tc_kernel."""
+    s = re.sub(r"^_ZN5llmlb|^_Z", "", mangled)
+    m = re.match(r"\d+", s)
+    return s[m.end(): m.end() + int(m.group())] if m else mangled
+
+
+FOLD_KERNELS = ("rmsnorm_parts_kernel", "rmsnorm_parts_cluster_kernel")
+
+
 def classes(log):
     """{context: set of launch classes}: ("gemm_tc_kernel" | "gemm_tc2_kernel", BN, EPI, K-split) for the projections,
     ("decode", cluster size) for decode attention (1 = the unsplit tensor-core kernel), ("prefill", kernel),
-    ("gemv_ks", B, EPI, NORM, CW, TW) for the K-split GEMV and ("gemv", B, EPI, NORM) for the row-owner GEMV."""
+    ("gemv_ks", B, EPI, NORM, CW, TW) for the K-split GEMV, ("gemv", B, EPI, NORM) for the row-owner GEMV,
+    ("fold", kernel, n_parts, gain, H) for the residual fold, ("rope", n_heads, n_kv), ("rmsnorm_kernel", H) and
+    ("embed_kernel", H)."""
     out, ctx = collections.defaultdict(set), "init"
     for line in open(log):
         if line.startswith("###"):
             ctx = line[4:].strip()
             continue
         p = line.split()
+        name = short_name(p[0])
+        if name in FOLD_KERNELS:
+            assert len(p) == 15, line            # n_parts, gain given, hidden appended
+            out[ctx].add(("fold", name, int(p[12]), p[13] == "1", int(p[14])))
+            continue
+        if name == "rope_append_kernel":
+            assert len(p) == 14, line            # n_heads, n_kv appended
+            out[ctx].add(("rope", int(p[12]), int(p[13])))
+            continue
+        if name in ("rmsnorm_kernel", "embed_kernel"):
+            assert len(p) == 13, line            # hidden appended
+            out[ctx].add((name, int(p[12])))
+            continue
         m = GEMM_RE.search(p[0])
         if m:
             assert len(p) == 13, line            # the fake runtime appends split_k to projection launches
@@ -72,12 +104,17 @@ def classes(log):
     return out
 
 
-def run_logged(tmp_path, name, argv, extra_env=None):
+def launched_kernels(tmp_path, name):
+    """The kernel names of every launch in the log run_logged(tmp_path, name, ...) wrote."""
+    return {short_name(l.split()[0]) for l in open(str(tmp_path / (name + ".log"))) if not l.startswith("###")}
+
+
+def run_logged(tmp_path, name, argv, extra_env=None, parse=classes):
     log = str(tmp_path / (name + ".log"))
     env = dict(os.environ, LD_PRELOAD=HL.build_fake(), FAKE_CUDART_LAUNCH_LOG=log, **(extra_env or {}))
     r = subprocess.run([sys.executable] + argv, env=env, capture_output=True, text=True, timeout=900)
     assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-3000:]
-    return classes(log)
+    return parse(log)
 
 
 def test_case_table_spans_the_dispatch_boundaries():
@@ -460,3 +497,225 @@ def test_gemv_bound_rejects_another_tokens_rms_scale(epi):
 def test_gemv_probe_rejects_a_gain_shifted_by_8(epi):
     assert _probe_rejects(epi, True, gain_shift=8) > 0
     assert _probe_rejects(epi, True, gain_shift=-8) > 0
+
+
+# ---------------------------------------------------------------------------- wide-step kernels: fold, norm, RoPE, embed --
+# Kernels of the tp = 1 launch plans that none of the case sweeps launches, with the tests that run them on the GPU.  A
+# kernel that appears in the plans and is neither launched by a GPU kernel test case nor listed here fails
+# test_every_kernel_of_the_launch_plans_is_gpu_tested_or_classified.
+COVERED_ELSEWHERE = {
+    "rope_table_kernel": "test_rope_scaling_gpu.py (the scaled table against fp64 up to position 131071)",
+    "sample_kernel": "test_ops_gpu.py (sampling against oracle.sampling_ref)",
+    "slot_init_kernel": "the engine tests (test_engine_gpu.py, test_parity_8b_gpu.py): step bookkeeping",
+    "prefill_finish_kernel": "the engine tests: step bookkeeping",
+    "step_finish_kernel": "the engine tests: step bookkeeping",
+    "sample_prepare_kernel": "the engine tests: step bookkeeping",
+    "decode_prepare_kernel": "the engine tests: step bookkeeping",
+    "iota_kernel": "the engine tests: step bookkeeping",
+    "fill_bf16_kernel": "the engine tests: weight set-up",
+    "synth_strided_kernel": "the engine tests: synthetic weights (test_engine_gpu.py checks them against the oracle generator)",
+    "gather_rows_kernel": "the engine tests: the rows that need logits",
+}
+STEP_KINDS = ("fold", "rope", "rmsnorm_kernel", "embed_kernel")
+PLAN_MODELS = ("8b", "mid", "70b")
+
+
+def _step_case_plan(tmp_path):
+    spec = tmp_path / "step_cases.json"
+    spec.write_text(json.dumps({
+        "fold": [[T, H, n, int(g), T * H + (SK.STRIDE_PAD if pad else 0)] for T, H, n, g, pad in SK.FOLD_CASES],
+        "rmsnorm": [list(c) for c in SK.RMSNORM_CASES],
+        "rope": [[T, nh, nkv] for nh, nkv in SK.ROPE_HEADS for T in SK.ROPE_TOKENS],
+        "embed": [[T, H, SK.EMBED_VOCAB] for T, H in SK.EMBED_CASES]}))
+    return run_logged(tmp_path, "step_cases", [os.path.join(HERE, "support", "kernel_case_sweep.py"), str(spec)])
+
+
+def _engine_plan(tmp_path, model, tp, max_width=None, parse=classes):
+    argv = [os.path.join(HERE, "support", "launch_plan_sweep.py"), model, str(tp)] + ([str(max_width)] if max_width else [])
+    return run_logged(tmp_path, "engine_%s_tp%d" % (model, tp), argv, parse=parse)
+
+
+def rope_shapes(log):
+    """{("rope", n_heads, n_kv)} of the rope_append_kernel launches in a log (of any tensor-parallel degree)."""
+    return {("rope", int(p[12]), int(p[13])) for p in (l.split() for l in open(log) if not l.startswith("###"))
+            if short_name(p[0]) == "rope_append_kernel"}
+
+
+def _kind(per_ctx, kinds=STEP_KINDS):
+    return {c for cs in per_ctx.values() for c in cs if c[0] in kinds}
+
+
+def test_step_case_tables_span_the_dispatch_boundaries():
+    Ts = {c[0] for c in SK.FOLD_CASES}
+    assert {T for T in Ts if T <= SK.CLUSTER_MAX_TOKENS} and {T for T in Ts if T > SK.CLUSTER_MAX_TOKENS}
+    assert {255, 256, 257} <= Ts and {c[2] for c in SK.FOLD_CASES} == {0, 1, 2, 4, 8}
+    assert {(c[3], c[4]) for c in SK.FOLD_CASES if c[2] >= 2} == {(g, p) for g in (False, True) for p in (False, True)}
+    assert SK.STRIDE_PAD % 4 == 0 and all(SK.STRIDE_PAD % H for H in SK.HIDDENS)
+    assert max(max(SK.rope_layout(T)[0]) for T in SK.ROPE_TOKENS) == SK.ROPE_MAX_POS - 1
+    slots = {p % 64 for T in SK.ROPE_TOKENS for p in SK.rope_layout(T)[0]}
+    assert {0, 63} <= slots
+    assert any(-1 in SK.rope_pages(*SK.rope_layout(T), 1)[0] for T in SK.ROPE_TOKENS)
+
+
+def test_gpu_step_kernel_cases_launch_every_class_the_engine_launches(built_lib, tmp_path):
+    """Every (kernel, n_parts, gain, H) of the residual fold, (n_heads, n_kv) of RoPE and H of the final RMSNorm and the
+    embedding that the tp = 1 engine launches at Llama-3-8B, LLAMA_MID and Llama-3-70B shapes over prefill widths 1..2048
+    (so the one-CTA-per-row fold above 256 rows is seen) must be among the classes the GPU step-kernel cases launch; and
+    so must the RoPE head shapes of the tensor-parallel shards of 8B and 70B at tp 2, 4 and 8."""
+    tested = _kind(_step_case_plan(tmp_path))
+    engine = {}
+    for model in PLAN_MODELS:
+        for c in _kind(_engine_plan(tmp_path, model, 1)):
+            engine.setdefault(c, model)
+    folds = {c for c in engine if c[0] == "fold"}
+    assert {c[1] for c in folds} == set(FOLD_KERNELS) and {c[4] for c in folds} == {2048, 4096, 8192}, sorted(folds)
+    assert ("fold", "rmsnorm_parts_cluster_kernel", 4, False, 4096) in folds                 # the last fold of 8B: no gain
+    assert ("fold", "rmsnorm_parts_cluster_kernel", 8, True, 2048) in folds                  # LLAMA_MID: 8 parts
+    missing = sorted((c, model) for c, model in engine.items() if c not in tested)
+    assert not missing, "the engine launches step-kernel classes no GPU test runs (class, model): %s" % missing
+    shards = set()
+    for model in ("8b", "70b"):
+        for tp in (2, 4, 8):
+            shards |= _engine_plan(tmp_path, model, tp, 8, parse=rope_shapes)
+    assert shards == {("rope", 32 // t, 8 // t) for t in (2, 4, 8)} | {("rope", 64 // t, 8 // t) for t in (2, 4, 8)}, sorted(shards)
+    missing = sorted(shards - tested)
+    assert not missing, "the tensor-parallel engine launches RoPE head shapes no GPU test runs: %s" % missing
+
+
+def test_every_kernel_of_the_launch_plans_is_gpu_tested_or_classified(built_lib, tmp_path):
+    """Every kernel the tp = 1 engine launches (8B, LLAMA_MID, 70B) is launched by a GPU kernel test case (GEMMs,
+    attention, GEMVs, step kernels) or is listed in COVERED_ELSEWHERE with the test that covers it.  A kernel added to
+    the engine fails here until someone classifies it."""
+    cases = {"gemm": [[T, N, Kd, e] for T, N, Kd, epis in K.GEMM_CASES for e in epis],
+             "wave_tail": list(K.WAVE_TAIL_CASE) + [K.wave_tail_rows(*K.WAVE_TAIL_CASE[:2])],
+             "decode_splits": K.DECODE_SPLITS, "max_split": K.GEMM_MAX_SPLIT}
+    spec = tmp_path / "cases.json"
+    spec.write_text(json.dumps(cases))
+    run_logged(tmp_path, "cases", [os.path.join(HERE, "support", "kernel_case_sweep.py"), str(spec)])
+    _gemv_sweep(tmp_path, "gemv_cases", GV.gemv_params())
+    _step_case_plan(tmp_path)
+    tested = set().union(*(launched_kernels(tmp_path, n) for n in ("cases", "gemv_cases", "step_cases")))
+    engine = set()
+    for model in PLAN_MODELS:
+        _engine_plan(tmp_path, model, 1)
+        engine |= launched_kernels(tmp_path, "engine_%s_tp1" % model)
+    assert len(engine) >= 20 and "?" not in engine, sorted(engine)
+    unclassified = sorted(engine - tested - set(COVERED_ELSEWHERE))
+    assert not unclassified, "kernels the engine launches that no GPU kernel test case runs and nobody classified: %s" % unclassified
+    stale = sorted(set(COVERED_ELSEWHERE) - engine)
+    assert not stale, "COVERED_ELSEWHERE names kernels the engine no longer launches: %s" % stale
+    assert not set(COVERED_ELSEWHERE) & tested, sorted(set(COVERED_ELSEWHERE) & tested)
+
+
+# teeth: the fold, norm and RoPE checkers applied on the CPU to outputs that are wrong in the ways these kernels go wrong
+FT, FH = 17, 2048          # a cluster-kernel step: each CTA owns a quarter (512 columns) of the row
+
+
+def _fold_case(n_parts=4):
+    return SK.fold_inputs(FT, FH, n_parts, 5, "cpu")
+
+
+def _norm_model(xf, gain, eps, gain_shift=0, quarter_ss=False, rs_from=None):
+    """y = bf16(x r g) in fp32 per token, as the kernels compute it, or wrong in one way."""
+    ss = (xf * xf).sum(-1, keepdim=True)
+    r = torch.rsqrt(ss / FH + torch.tensor(eps, dtype=torch.float32))
+    if quarter_ss:          # each CTA normalises its quarter by its own partial sum: no DSMEM exchange
+        q = FH // 4
+        r = torch.cat([torch.rsqrt((xf[:, i * q:(i + 1) * q] ** 2).sum(-1, keepdim=True) / FH + eps).expand(-1, q) for i in range(4)], 1)
+    if rs_from is not None:
+        r = r[rs_from]
+    return (xf * r * gain.float().roll(-gain_shift)).to(torch.bfloat16)
+
+
+def _norm_rejects(**knobs):
+    x, parts, g = _fold_case()
+    xf = SK.fold_ref(x, parts)
+    return SK.check_norm(_norm_model(xf, g, SK.EPS, **knobs), xf, g, SK.EPS, FH, True)[0]
+
+
+def test_fold_and_norm_checkers_accept_a_correct_kernel():
+    x, parts, g = _fold_case()
+    assert K.bits_equal(SK.fold_ref(x, parts), SK.fold_ref(x.clone(), [p.clone() for p in parts])) == 0
+    assert _norm_rejects() == 0
+    for cluster in (False, True):
+        for H in SK.HIDDENS:
+            assert 2.0 ** -21 < SK.norm_rel_bound(H, cluster) < 2.0 ** -18
+
+
+def test_fold_checker_rejects_a_dropped_last_part_and_the_reverse_order():
+    x, parts, g = _fold_case()
+    want = SK.fold_ref(x, parts)
+    assert K.bits_equal(SK.fold_ref(x, parts[:-1]), want) > 0
+    assert K.bits_equal(SK.fold_ref(x, parts[::-1]), want) > 0
+
+
+def test_norm_checker_rejects_a_gain_one_quarter_off_a_missing_exchange_and_another_tokens_scale():
+    assert _norm_rejects(gain_shift=FH // 4) > 0
+    assert _norm_rejects(gain_shift=-FH // 4) > 0
+    assert _norm_rejects(quarter_ss=True) > 0
+    assert _norm_rejects(rs_from=[(t + 1) % FT for t in range(FT)]) > 0
+
+
+_TABLE = {}
+
+
+def _rope_table():
+    """The Llama 3.1 table, fp64 angles rounded to fp32 (what rope_table_kernel computes)."""
+    if not _TABLE:
+        from rope_oracle import rope_freq_factors
+        from rope_scaling_util import LLAMA31_8B, THETA
+        f = torch.tensor(rope_freq_factors(LLAMA31_8B, THETA), dtype=torch.float32).double()
+        inv = torch.pow(torch.tensor(THETA, dtype=torch.float32).double(), -torch.arange(0, 128, 2).double() / 128) / f
+        ang = torch.arange(SK.ROPE_MAX_POS).double()[:, None] * inv[None]
+        _TABLE[0] = torch.stack([ang.cos(), ang.sin()], -1).float()
+    return _TABLE[0]
+
+
+RT, RNH, RNKV = 65, 8, 2
+
+
+def _rope_case():
+    pos_l, seq = SK.rope_layout(RT)
+    page_l, n_pages = SK.rope_pages(pos_l, seq, 3)
+    gen = torch.Generator().manual_seed(4)
+    qkv = (torch.randn(RT, (RNH + 2 * RNKV) * 128, generator=gen) * 4).to(torch.bfloat16)
+    pool = torch.full((n_pages, RNKV, 64, 128), float("nan"), dtype=torch.bfloat16)
+    return qkv, torch.tensor(pos_l, dtype=torch.int32), torch.tensor(page_l, dtype=torch.int32), pool
+
+
+def _rope_model(qkv, pos, page, pool, pair_stride=64, pos_shift=0, sin_sign=1.0, slot_shift=0):
+    """rope_append in fp32 on the CPU, right or wrong in one way: returns (qkv out, K pool, V pool)."""
+    tab = _rope_table()
+    nr = RNH + RNKV
+    x = qkv[:, : nr * 128].reshape(RT, nr, 128).float()
+    cs = tab[(pos.long() + pos_shift).clamp(min=0)]
+    c, s = cs[:, None, :, 0], sin_sign * cs[:, None, :, 1]
+    if pair_stride == 64:
+        a, b = x[..., :64], x[..., 64:]
+    else:                                   # pairs (2i, 2i + 1)
+        a, b = x[..., 0::2], x[..., 1::2]
+    ra, rb = a * c - b * s, b * c + a * s
+    rot = torch.cat([ra, rb], -1) if pair_stride == 64 else torch.stack([ra, rb], -1).flatten(-2)
+    out = qkv.clone()
+    out[:, : nr * 128] = rot.reshape(RT, nr * 128).to(torch.bfloat16)
+    kp, vp = SK.rope_pool_expected(pool, pool, qkv, out, pos + slot_shift, page, RNH, RNKV)
+    return out, kp, vp
+
+
+def _rope_rejects(**knobs):
+    qkv, pos, page, pool = _rope_case()
+    out, kp, vp = _rope_model(qkv, pos, page, pool, **knobs)
+    n_bad, _ = SK.rope_check(qkv, out, pos, _rope_table(), RNH, RNKV)
+    kw, vw = SK.rope_pool_expected(pool, pool, qkv, out, pos, page, RNH, RNKV)
+    return n_bad + K.bits_equal(kp, kw) + K.bits_equal(vp, vw)
+
+
+def test_rope_checker_accepts_a_correct_kernel():
+    assert _rope_rejects() == 0
+
+
+def test_rope_checker_rejects_wrong_pairs_positions_sin_sign_and_slot():
+    assert _rope_rejects(pair_stride=1) > 0
+    assert _rope_rejects(pos_shift=-1) > 0
+    assert _rope_rejects(sin_sign=-1.0) > 0
+    assert _rope_rejects(slot_shift=1) > 0

@@ -32,3 +32,19 @@ def test_hopper_mnemonics_present(built_lib, obj):
         assert n >= least, "%s: %s occurs %d times, expected >= %d" % (obj, pat, n, least)
     if obj in ("gemm_tc.o", "gemm_tc2.o", "attention_tc.o"):
         assert not re.search(r"\bHMMA\b", sass), obj    # the wgmma kernels carry no mma.sync
+
+
+@pytest.mark.skipif(shutil.which("cuobjdump") is None, reason="cuobjdump not on PATH")
+def test_cluster_rmsnorm_waits_for_its_peers_before_storing_into_their_shared_memory(built_lib):
+    """rmsnorm_parts_cluster_kernel stores its partial sum of squares into the three peer CTAs' shared memory
+    (st.shared::cluster: SASS ST.E to a mapa address).  A CTA may only do that once every CTA of the cluster is running, so
+    a cluster barrier wait (UCGABAR_WAIT) must come before the first such store."""
+    sass = subprocess.run(["cuobjdump", "-sass", os.path.join(ROOT, "llmlb_b200", "_build", "elementwise.o")], capture_output=True,
+                          text=True, timeout=600).stdout
+    fns = [f for f in re.split(r"\n\s*Function : ", sass)[1:] if f.split("\n", 1)[0].strip().startswith("_ZN5llmlb28rmsnorm_parts_cluster_kernel")]
+    assert len(fns) == 1, "rmsnorm_parts_cluster_kernel not found in elementwise.o"
+    lines = fns[0].splitlines()
+    store = next((i for i, l in enumerate(lines) if re.search(r"\bST\.E\b", l)), None)
+    wait = next((i for i, l in enumerate(lines) if "UCGABAR_WAIT" in l), None)
+    assert store is not None, "no remote shared-memory store found"
+    assert wait is not None and wait < store, "the first remote store (line %d) comes before any cluster barrier wait (%s)" % (store, wait)
