@@ -48,7 +48,14 @@ pub enum LocalBody {
     Sse(std::pin::Pin<Box<dyn Stream<Item = Result<Bytes, std::io::Error>> + Send>>),
 }
 
+/// `frequency_penalty`, `presence_penalty` (null or absent: 0) and `logit_bias` ({"token id": value}) as OpenAI sends them;
+/// a bias key that is not a decimal token id is kept as -1, which the engine refuses with a 400 naming the field.
 fn sampling_from(payload: &Value, max_key: &str, stop_ids: Vec<i32>) -> Sampling {
+    let logit_bias = payload
+        .get("logit_bias")
+        .and_then(Value::as_object)
+        .map(|m| m.iter().map(|(k, v)| (k.parse::<i32>().unwrap_or(-1), v.as_f64().unwrap_or(f64::NAN) as f32)).collect())
+        .unwrap_or_default();
     Sampling {
         max_tokens: payload.get(max_key).and_then(Value::as_u64).unwrap_or(128).max(1) as u32,
         temperature: payload.get("temperature").and_then(Value::as_f64).unwrap_or(1.0) as f32,
@@ -57,6 +64,9 @@ fn sampling_from(payload: &Value, max_key: &str, stop_ids: Vec<i32>) -> Sampling
         seed: payload.get("seed").and_then(Value::as_u64).unwrap_or(0),
         stop_ids,
         ignore_eos: false,
+        frequency_penalty: payload.get("frequency_penalty").and_then(Value::as_f64).unwrap_or(0.0) as f32,
+        presence_penalty: payload.get("presence_penalty").and_then(Value::as_f64).unwrap_or(0.0) as f32,
+        logit_bias,
     }
 }
 

@@ -118,6 +118,17 @@ pub struct llmlb_sampling {
     pub ignore_eos: u32,
 }
 
+/// OpenAI's frequency_penalty, presence_penalty and logit_bias (`llmlb_request_submit_penalized`).
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct llmlb_penalties {
+    pub frequency_penalty: f32,
+    pub presence_penalty: f32,
+    pub bias_ids: *const i32,
+    pub bias_values: *const f32,
+    pub n_bias: u32,
+}
+
 #[repr(C)]
 #[derive(Clone, Copy, Debug, Default)]
 pub struct llmlb_token_event {
@@ -143,6 +154,7 @@ extern "C" {
     pub fn llmlb_engine_tp_plan_channel(e: *mut llmlb_engine, shm_name: *const c_char) -> c_int;
     pub fn llmlb_engine_pause(e: *mut llmlb_engine, paused: u32) -> c_int;
     pub fn llmlb_request_submit(e: *mut llmlb_engine, prompt_ids: *const i32, n_prompt: u32, s: *const llmlb_sampling, req_id: *mut u64) -> c_int;
+    pub fn llmlb_request_submit_penalized(e: *mut llmlb_engine, prompt_ids: *const i32, n_prompt: u32, s: *const llmlb_sampling, pen: *const llmlb_penalties, req_id: *mut u64) -> c_int;
     pub fn llmlb_request_poll(e: *mut llmlb_engine, req_id: u64, out: *mut llmlb_token_event, cap: u32, n_out: *mut u32, timeout_ms: c_int) -> c_int;
     pub fn llmlb_request_cancel(e: *mut llmlb_engine, req_id: u64) -> c_int;
     pub fn llmlb_request_release(e: *mut llmlb_engine, req_id: u64) -> c_int;
@@ -206,11 +218,16 @@ pub struct Sampling {
     pub seed: u64,
     pub stop_ids: Vec<i32>,
     pub ignore_eos: bool,
+    /// OpenAI penalties, applied on the device before sampling; both 0 and no bias: not penalised
+    pub frequency_penalty: f32,
+    pub presence_penalty: f32,
+    pub logit_bias: Vec<(i32, f32)>,
 }
 
 impl Default for Sampling {
     fn default() -> Self {
-        Self { max_tokens: 128, temperature: 1.0, top_k: 0, top_p: 1.0, seed: 0, stop_ids: Vec::new(), ignore_eos: false }
+        Self { max_tokens: 128, temperature: 1.0, top_k: 0, top_p: 1.0, seed: 0, stop_ids: Vec::new(), ignore_eos: false,
+               frequency_penalty: 0.0, presence_penalty: 0.0, logit_bias: Vec::new() }
     }
 }
 
@@ -271,7 +288,20 @@ impl Engine {
             ignore_eos: s.ignore_eos as u32,
         };
         let mut id = 0u64;
-        check(unsafe { llmlb_request_submit(self.raw, prompt_ids.as_ptr(), prompt_ids.len() as u32, &raw_s, &mut id) })?;
+        if s.frequency_penalty == 0.0 && s.presence_penalty == 0.0 && s.logit_bias.is_empty() {
+            check(unsafe { llmlb_request_submit(self.raw, prompt_ids.as_ptr(), prompt_ids.len() as u32, &raw_s, &mut id) })?;
+            return Ok(id);
+        }
+        let ids: Vec<i32> = s.logit_bias.iter().map(|b| b.0).collect();
+        let vals: Vec<f32> = s.logit_bias.iter().map(|b| b.1).collect();
+        let pen = llmlb_penalties {
+            frequency_penalty: s.frequency_penalty,
+            presence_penalty: s.presence_penalty,
+            bias_ids: if ids.is_empty() { std::ptr::null() } else { ids.as_ptr() },
+            bias_values: if vals.is_empty() { std::ptr::null() } else { vals.as_ptr() },
+            n_bias: ids.len() as u32,
+        };
+        check(unsafe { llmlb_request_submit_penalized(self.raw, prompt_ids.as_ptr(), prompt_ids.len() as u32, &raw_s, &pen, &mut id) })?;
         Ok(id)
     }
 

@@ -184,6 +184,24 @@ typedef struct llmlb_token_event {
 /* Non-blocking enqueue; prompt_ids are copied.  */
 int llmlb_request_submit(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt,
                          const llmlb_sampling* s, uint64_t* req_id);
+
+/* OpenAI's frequency_penalty, presence_penalty and logit_bias.  Before sampling, every logit of the request becomes
+ *   z[j] = (logit[j] - (c[j] * frequency_penalty + (c[j] > 0 ? presence_penalty : 0))) + bias[j]
+ * (fp32, in this order), c[j] = times token j was generated by this request so far (not the prompt; tokens generated
+ * before a preemption count), bias[j] = 0 for ids not in the list.  Temperature, top-k and top-p then apply to z. */
+#define LLMLB_MAX_LOGIT_BIAS 1024
+typedef struct llmlb_penalties {
+  float frequency_penalty;         /* finite, in [-2, 2] */
+  float presence_penalty;          /* finite, in [-2, 2] */
+  const int32_t* bias_ids;         /* distinct ids in [0, vocab) */
+  const float* bias_values;        /* finite, in [-100, 100] */
+  uint32_t n_bias;                 /* <= LLMLB_MAX_LOGIT_BIAS */
+} llmlb_penalties;
+/* llmlb_request_submit with penalties (NULL = none; the bias list is copied).  Out-of-range values return
+ * LLMLB_E_INVALID_ARG, and the error text names the field.  A request with both penalties 0 and no bias is not
+ * penalised: it runs exactly as through llmlb_request_submit. */
+int llmlb_request_submit_penalized(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt,
+                                   const llmlb_sampling* s, const llmlb_penalties* pen, uint64_t* req_id);
 /* Drain up to cap events. timeout_ms: 0 = return at once, <0 = wait until at least one. */
 int llmlb_request_poll(llmlb_engine* e, uint64_t req_id, llmlb_token_event* out, uint32_t cap,
                        uint32_t* n_out, int timeout_ms);
@@ -291,6 +309,13 @@ int llmlb_op_decode_attention(const void* qkv_bf16, void* k_pages, void* v_pages
 int llmlb_op_sample(const float* logits, uint32_t n_rows, uint32_t vocab, const float* temperature,
                     const float* top_p, const int32_t* top_k, const uint64_t* seed,
                     const uint64_t* step, int32_t* out_ids, void* stream);
+/* a2.12 penalties, in place before llmlb_op_sample (the kernel the engine launches; formula at llmlb_penalties).
+ * Row r reads counts + r*count_stride (int32 [vocab]), freq[r], pres[r], n_bias[r] and its bias list at
+ * bias_ids / bias_vals + r*bias_stride (n_bias[r] <= bias_stride <= LLMLB_MAX_LOGIT_BIAS, distinct ids in [0, vocab)).
+ * A row with freq = pres = 0 and no bias is left unchanged. */
+int llmlb_op_penalize(float* logits, uint32_t n_rows, uint32_t vocab, const int32_t* counts, uint64_t count_stride,
+                      const float* freq, const float* pres, const int32_t* bias_ids, const float* bias_vals,
+                      const uint32_t* n_bias, uint32_t bias_stride, void* stream);
 /* a2.13 all-reduce(sum) of fp32 [n] across tp ranks through peer-mapped buffers. */
 int llmlb_op_allreduce(llmlb_engine* e, float* buf_f32, uint64_t n, void* stream);
 

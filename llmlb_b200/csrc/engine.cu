@@ -5,8 +5,9 @@
 // iteration-level continuous-batching scheduler on its own thread (SURVEY §8 a2.14), per-request
 // token-event queues for non-blocking submit/poll/cancel.  Device side: the kernels in the
 // sibling .cu files, chained on one stream; decode steps are captured into CUDA graphs per batch
-// width and all per-sequence decode state (length, last token, sampler counters) lives in HBM so
-// the GPU never waits for the host between tokens — the host reads tokens `lookahead` steps late.
+// width and all per-sequence decode state (length, last token, sampler counters, the token counts
+// and bias list of frequency / presence penalties) lives in HBM so the GPU never waits for the
+// host between tokens — the host reads tokens `lookahead` steps late.
 #include <cuda.h>
 
 #include <algorithm>
@@ -72,6 +73,13 @@ int make_tmap_attn_kv(CUtensorMap* m, const void* pool, uint64_t n_layers, uint6
 int prefill_attention_tc_launch(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, uint32_t layer,
                                 const int32_t* block_tables, uint32_t bt_stride, const int32_t* tiles, uint32_t n_tiles,
                                 void* out, uint32_t n_heads, uint32_t n_kv, bool pdl, cudaStream_t st);
+int penalize_launch(float* logits, uint32_t n_rows, uint32_t vocab, const int32_t* counts, uint64_t count_stride,
+                    const float* freq, const float* pres, const int32_t* bias_ids, const float* bias_vals,
+                    const uint32_t* n_bias, uint32_t bias_stride, const int32_t* row_slot, cudaStream_t st);
+int penalty_count_launch(int32_t* counts, uint64_t count_stride, const float* freq, const float* pres, const uint32_t* n_bias,
+                         const int32_t* row_slot, const int32_t* out_ids, uint32_t n_rows, cudaStream_t st);
+int penalty_reset_launch(int32_t* counts, uint64_t count_stride, float* freq, float* pres, uint32_t* n_bias, int32_t slot,
+                         float f, float p, uint32_t nb, uint32_t vocab, const int32_t* gen, uint32_t n_gen, cudaStream_t st);
 int rope_append_launch(void* qkv, const int32_t* positions, const int32_t* page_of_token, const float* rope_table,
                        void* k_pages, void* v_pages, uint32_t n_tokens, uint32_t n_heads, uint32_t n_kv, bool pdl,
                        cudaStream_t st);
@@ -113,6 +121,9 @@ struct SlotState {  // per-sequence decode state, device resident
   int32_t* top_k;
   uint64_t* seed;
   uint64_t* step;
+  float* pen_freq;      // penalties (penalty.cu): both 0 and no bias = the slot is not penalised
+  float* pen_pres;
+  uint32_t* pen_n_bias;
 };
 struct BatchView {  // compact per-step arrays
   int32_t* slots;     // batch position -> slot
@@ -173,6 +184,10 @@ struct Request {
   std::vector<int32_t> prompt;
   llmlb_sampling s{};
   std::vector<int32_t> stop_ids;
+  bool penalized = false;   // frequency / presence penalty or logit bias (penalty.cu)
+  float freq_pen = 0.f, pres_pen = 0.f;
+  std::vector<int32_t> bias_ids;
+  std::vector<float> bias_vals;
   int slot = -1;
   std::vector<int32_t> pages;
   uint32_t prefilled = 0;   // context tokens whose KV is (being) written
@@ -372,6 +387,12 @@ struct llmlb_engine {
           *d_last_rows = nullptr;
   SlotState S{};
   BatchView B{};
+  // penalties: int32 token counts [max_seqs][vocab] and bias lists [max_seqs][LLMLB_MAX_LOGIT_BIAS] per slot, and the
+  // generated tokens of a re-admitted sequence [max_ctx] on their way to penalty_reset_kernel
+  int32_t* pen_counts = nullptr;
+  int32_t* pen_bias_ids = nullptr;
+  float* pen_bias_vals = nullptr;
+  int32_t* pen_gen = nullptr;
   static constexpr int kRing = 8;
   uint8_t* h_stage[kRing] = {};
   size_t stage_bytes = 0;
@@ -395,7 +416,7 @@ struct llmlb_engine {
   __nv_bfloat16* ylast = nullptr;    // [max_seqs][hidden] normalised rows that need logits (protocol B)
   CUtensorMap m_ylast[5]{};
 
-  // decode graphs by batch width
+  // decode graphs by batch width, with bit 31 set when some sequence of the batch is penalised
   std::unordered_map<uint32_t, cudaGraphExec_t> graphs;
   std::unordered_map<uint32_t, uint64_t> graph_nodes;  // kernels per captured step
   bool paused = false;
@@ -446,8 +467,10 @@ struct llmlb_engine {
   };
   int proj(const CUtensorMap& mw, const void* w, const void* xin, const CUtensorMap* mx, void* out, uint32_t T,
            uint32_t n_out, uint32_t k, uint32_t epi, uint32_t out_stride, int wait_coll = -1);
-  int layer_stack_decode(uint32_t nb);
-  int launch_decode_step(uint32_t nb);
+  int layer_stack_decode(uint32_t nb, bool pen = false);
+  int launch_decode_step(uint32_t nb, bool pen);
+  int penalize_rows(uint32_t R);         // before sampling R rows of B (slots in B.slots)
+  int count_sampled(uint32_t R);         // after sampling: each penalised row's token counts
   int forward_tokens(uint32_t T, bool decode, uint32_t nb, uint32_t n_tiles, FwdState* fs);
   int forward_small_tp(uint32_t T, bool decode, uint32_t nb, uint32_t n_tiles, FwdState* fs);
   int forward_big_tp(uint32_t T, bool decode, uint32_t nb, uint32_t n_tiles, FwdState* fs);
@@ -686,6 +709,10 @@ int llmlb_engine::alloc_all() {
   const size_t ms = cfg.max_seqs;
   RC(dmalloc(&S.seq_len, ms)); RC(dmalloc(&S.last_token, ms)); RC(dmalloc(&S.temperature, ms));
   RC(dmalloc(&S.top_p, ms)); RC(dmalloc(&S.top_k, ms)); RC(dmalloc(&S.seed, ms)); RC(dmalloc(&S.step, ms));
+  RC(dmalloc(&S.pen_freq, ms)); RC(dmalloc(&S.pen_pres, ms)); RC(dmalloc(&S.pen_n_bias, ms));
+  RC(dmalloc(&pen_counts, ms * M.vocab));   // int32: a count can pass 65535 at 128K context
+  RC(dmalloc(&pen_bias_ids, ms * LLMLB_MAX_LOGIT_BIAS)); RC(dmalloc(&pen_bias_vals, ms * LLMLB_MAX_LOGIT_BIAS));
+  RC(dmalloc(&pen_gen, cfg.max_ctx));
   RC(dmalloc(&B.slots, ms)); RC(dmalloc(&B.ids, ms)); RC(dmalloc(&B.seq_lens, ms));
   RC(dmalloc(&B.temperature, ms)); RC(dmalloc(&B.top_p, ms)); RC(dmalloc(&B.top_k, ms));
   RC(dmalloc(&B.seed, ms)); RC(dmalloc(&B.step, ms)); RC(dmalloc(&B.out_ids, ms));
@@ -983,41 +1010,53 @@ int llmlb_engine::logits_after_forward(FwdState* fs, uint32_t R, bool decode) {
   return LLMLB_E_INTERNAL;   // prefill with fp32 residual: run_prefill gathers the rows itself
 }
 
-int llmlb_engine::layer_stack_decode(uint32_t nb) {
+int llmlb_engine::penalize_rows(uint32_t R) {
+  return penalize_launch(logits, R, M.vocab, pen_counts, M.vocab, S.pen_freq, S.pen_pres, pen_bias_ids, pen_bias_vals,
+                         S.pen_n_bias, LLMLB_MAX_LOGIT_BIAS, B.slots, st);
+}
+int llmlb_engine::count_sampled(uint32_t R) {
+  return penalty_count_launch(pen_counts, M.vocab, S.pen_freq, S.pen_pres, S.pen_n_bias, B.slots, B.out_ids, R, st);
+}
+
+// pen: some sequence of the batch is penalised (the unpenalised step launches exactly what it did without penalties)
+int llmlb_engine::layer_stack_decode(uint32_t nb, bool pen) {
   decode_prepare_kernel<<<ceil_div(nb, 128), 128, 0, st>>>(S, B, nb);
   LLMLB_LAUNCH_CHECK();
   RC(llmlb_op_embed(embed, B.ids, x, nb, M.hidden, M.vocab, st));
   FwdState fs;
   RC(forward_tokens(nb, true, nb, 0, &fs));
   RC(logits_after_forward(&fs, nb, true));
+  if (pen) RC(penalize_rows(nb));
   RC(llmlb_op_sample(logits, nb, M.vocab, B.temperature, B.top_p, B.top_k, B.seed, B.step, B.out_ids, st));
   step_finish_kernel<<<ceil_div(nb, 128), 128, 0, st>>>(S, B, nb);
   LLMLB_LAUNCH_CHECK();
+  if (pen) RC(count_sampled(nb));
   return LLMLB_OK;
 }
 
-int llmlb_engine::launch_decode_step(uint32_t nb) {
-  if (!cfg.use_cuda_graphs) return layer_stack_decode(nb);
-  auto it = graphs.find(nb);
+int llmlb_engine::launch_decode_step(uint32_t nb, bool pen) {
+  if (!cfg.use_cuda_graphs) return layer_stack_decode(nb, pen);
+  const uint32_t key = nb | (pen ? 0x80000000u : 0u);
+  auto it = graphs.find(key);
   if (it == graphs.end()) {
     // kernel attributes (max dynamic smem) were set by the eager warm-up in init()
     cudaGraph_t g = nullptr;
     uint64_t launches_before = g_kernel_launches.load();
     LLMLB_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    int rc = layer_stack_decode(nb);
+    int rc = layer_stack_decode(nb, pen);
     cudaError_t ce = cudaStreamEndCapture(st, &g);
     if (rc != LLMLB_OK) { if (g) cudaGraphDestroy(g); return rc; }
     if (ce != cudaSuccess) { set_error(std::string("graph capture: ") + cudaGetErrorString(ce)); return LLMLB_E_DEVICE; }
     cudaGraphExec_t ge = nullptr;
     LLMLB_CUDA_CHECK(cudaGraphInstantiate(&ge, g, 0));
     cudaGraphDestroy(g);
-    graphs[nb] = ge;
-    graph_nodes[nb] = g_kernel_launches.load() - launches_before;
+    graphs[key] = ge;
+    graph_nodes[key] = g_kernel_launches.load() - launches_before;
     g_kernel_launches.store(launches_before);  // capture did not execute anything
-    it = graphs.find(nb);
+    it = graphs.find(key);
   }
   LLMLB_CUDA_CHECK(cudaGraphLaunch(it->second, st));
-  g_kernel_launches.fetch_add(graph_nodes[nb]);
+  g_kernel_launches.fetch_add(graph_nodes[key]);
   return LLMLB_OK;
 }
 
@@ -1035,6 +1074,9 @@ __global__ void slot_init_kernel(SlotState S, int32_t slot, float temperature, f
   S.top_k[slot] = top_k;
   S.seed[slot] = seed;
   S.step[slot] = step0;   // a preempted sequence resumes its sampler stream where it stopped
+  S.pen_freq[slot] = 0.f;  // unpenalised; penalty_reset_kernel follows for a penalised request
+  S.pen_pres[slot] = 0.f;
+  S.pen_n_bias[slot] = 0;
 }
 __global__ void prefill_finish_kernel(SlotState S, BatchView B, uint32_t n) {
   uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1072,6 +1114,7 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
   step.is_prefill = true;
   step.n_tokens = T;
   uint32_t row = 0, n_tiles = 0, R = 0;
+  bool pen_rows = false;   // some finished row is penalised
   for (size_t i = 0; i < reqs.size(); ++i) {
     Request& r = *reqs[i];
     if (r.prefilled == 0) {  // first chunk: publish block table + sampler state
@@ -1079,6 +1122,16 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
                                        r.pages.size() * 4, cudaMemcpyHostToDevice, st));
       slot_init_kernel<<<1, 1, 0, st>>>(S, r.slot, r.s.temperature, r.s.top_p, (int32_t)r.s.top_k, r.s.seed, uint64_t(r.harvested));
       LLMLB_LAUNCH_CHECK();
+      if (r.penalized) {   // bias list into the slot's rows; counts = the tokens generated before a preemption (none otherwise)
+        const uint32_t nb = uint32_t(r.bias_ids.size());
+        if (nb) {
+          LLMLB_CUDA_CHECK(cudaMemcpyAsync(pen_bias_ids + size_t(r.slot) * LLMLB_MAX_LOGIT_BIAS, r.bias_ids.data(), nb * 4, cudaMemcpyHostToDevice, st));
+          LLMLB_CUDA_CHECK(cudaMemcpyAsync(pen_bias_vals + size_t(r.slot) * LLMLB_MAX_LOGIT_BIAS, r.bias_vals.data(), nb * 4, cudaMemcpyHostToDevice, st));
+        }
+        if (!r.gen.empty()) LLMLB_CUDA_CHECK(cudaMemcpyAsync(pen_gen, r.gen.data(), r.gen.size() * 4, cudaMemcpyHostToDevice, st));
+        RC(penalty_reset_launch(pen_counts, M.vocab, S.pen_freq, S.pen_pres, S.pen_n_bias, r.slot, r.freq_pen, r.pres_pen, nb,
+                                M.vocab, pen_gen, uint32_t(r.gen.size()), st));
+      }
       r.pages_published = uint32_t(r.pages.size());
     }
     const uint32_t p0 = r.prefilled;
@@ -1099,6 +1152,7 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
       s_rows[R] = int32_t(row + take[i] - 1);
       s_slots[R] = r.slot;
       s_lens[R] = int32_t(r.prompt.size());
+      pen_rows |= r.penalized;
       step.reqs.push_back(reqs[i]);
       ++R;
     }
@@ -1132,9 +1186,11 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
     }
     sample_prepare_kernel<<<ceil_div(R, 128), 128, 0, st>>>(S, B, R);
     LLMLB_LAUNCH_CHECK();
+    if (pen_rows) RC(penalize_rows(R));
     RC(llmlb_op_sample(logits, R, M.vocab, B.temperature, B.top_p, B.top_k, B.seed, B.step, B.out_ids, st));
     step_finish_kernel<<<ceil_div(R, 128), 128, 0, st>>>(S, B, R);
     LLMLB_LAUNCH_CHECK();
+    if (pen_rows) RC(count_sampled(R));
     prefill_finish_kernel<<<ceil_div(R, 128), 128, 0, st>>>(S, B, R);
     LLMLB_LAUNCH_CHECK();
     step.host_ids = h_out[(out_seq++) % kRing];
@@ -1189,7 +1245,9 @@ int llmlb_engine::run_decode(const std::vector<ReqPtr>& batch) {
   step.ev_start = get_event();
   step.ev_end = get_event();
   LLMLB_CUDA_CHECK(cudaEventRecord(step.ev_start, st));
-  RC(launch_decode_step(nb));
+  bool pen = false;
+  for (auto& r : batch) pen |= r->penalized;
+  RC(launch_decode_step(nb, pen));
   step.host_ids = h_out[(out_seq++) % kRing];
   LLMLB_CUDA_CHECK(cudaMemcpyAsync(step.host_ids, B.out_ids, nb * 4, cudaMemcpyDeviceToHost, st));
   LLMLB_CUDA_CHECK(cudaEventRecord(step.ev_end, st));
@@ -1458,7 +1516,15 @@ void llmlb_engine::loop_follower() {
         r->n_prompt0 = n_prompt;
         p += size_t(n_prompt) * 4;
         r->stop_ids.assign(reinterpret_cast<const int32_t*>(p), reinterpret_cast<const int32_t*>(p) + n_stop);
+        p += size_t(n_stop) * 4;
         r->s.stop_ids = nullptr;
+        if (size_t(buf.data() + buf.size() - p) >= 12) {   // a penalised request
+          uint32_t n_bias = 0;
+          memcpy(&r->freq_pen, p, 4); memcpy(&r->pres_pen, p + 4, 4); memcpy(&n_bias, p + 8, 4); p += 12;
+          r->bias_ids.assign(reinterpret_cast<const int32_t*>(p), reinterpret_cast<const int32_t*>(p) + n_bias);
+          r->bias_vals.assign(reinterpret_cast<const float*>(p + size_t(n_bias) * 4), reinterpret_cast<const float*>(p + size_t(n_bias) * 8));
+          r->penalized = true;
+        }
         r->client_released = true;
         r->t_submit = std::chrono::steady_clock::now();
         std::lock_guard<std::mutex> lk(mu);
@@ -1548,6 +1614,7 @@ extern "C" void llmlb_engine_destroy(llmlb_engine* e) {
   F(e->x); if (e->tp == 1) F(e->y); F(e->xb); F(e->tp_stage); F(e->ylast); F(e->qkv); F(e->attn); F(e->h); F(e->logits); F(e->logits_l); F(e->x_last); F(e->attn_ws);
   F(e->d_ids); F(e->d_pos); F(e->d_page_of_tok); F(e->d_tiles); F(e->d_last_rows);
   F(e->S.seq_len); F(e->S.last_token); F(e->S.temperature); F(e->S.top_p); F(e->S.top_k); F(e->S.seed); F(e->S.step);
+  F(e->S.pen_freq); F(e->S.pen_pres); F(e->S.pen_n_bias); F(e->pen_counts); F(e->pen_bias_ids); F(e->pen_bias_vals); F(e->pen_gen);
   F(e->B.slots); F(e->B.ids); F(e->B.seq_lens); F(e->B.temperature); F(e->B.top_p); F(e->B.top_k);
   F(e->B.seed); F(e->B.step); F(e->B.out_ids);
   for (int i = 0; i < llmlb_engine::kRing; ++i) {
@@ -1598,9 +1665,45 @@ extern "C" int llmlb_engine_health(const llmlb_engine* ce, llmlb_health* out) {
   return LLMLB_OK;
 }
 
+// Checks a penalty set against the documented ranges and copies it into r (penalized stays false for a neutral set).
+static int take_penalties(const llmlb_penalties* pen, uint32_t vocab, Request* r) {
+  if (!pen) return LLMLB_OK;
+  const char* fn = "llmlb_request_submit_penalized: ";
+  auto bad = [&](const std::string& m) { set_error(fn + m); return LLMLB_E_INVALID_ARG; };
+  if (!std::isfinite(pen->frequency_penalty) || pen->frequency_penalty < -2.f || pen->frequency_penalty > 2.f)
+    return bad("frequency_penalty must be finite and in [-2, 2]");
+  if (!std::isfinite(pen->presence_penalty) || pen->presence_penalty < -2.f || pen->presence_penalty > 2.f)
+    return bad("presence_penalty must be finite and in [-2, 2]");
+  if (pen->n_bias > LLMLB_MAX_LOGIT_BIAS) return bad("logit_bias has more than 1024 entries");
+  if (pen->n_bias && (!pen->bias_ids || !pen->bias_values)) return bad("logit_bias: NULL ids or values with n_bias > 0");
+  std::vector<int32_t> ids(pen->bias_ids, pen->bias_ids + pen->n_bias);
+  for (uint32_t i = 0; i < pen->n_bias; ++i) {
+    if (ids[i] < 0 || uint32_t(ids[i]) >= vocab) return bad("logit_bias: token id " + std::to_string(ids[i]) + " outside the vocabulary");
+    const float v = pen->bias_values[i];
+    if (!std::isfinite(v) || v < -100.f || v > 100.f) return bad("logit_bias: value of token " + std::to_string(ids[i]) + " must be finite and in [-100, 100]");
+  }
+  std::sort(ids.begin(), ids.end());
+  if (std::adjacent_find(ids.begin(), ids.end()) != ids.end()) return bad("logit_bias: duplicate token id");
+  // +0 for -0: a zero penalty is no penalty, and the kernel tests it with != 0
+  r->freq_pen = pen->frequency_penalty == 0.f ? 0.f : pen->frequency_penalty;
+  r->pres_pen = pen->presence_penalty == 0.f ? 0.f : pen->presence_penalty;
+  r->bias_ids.assign(pen->bias_ids, pen->bias_ids + pen->n_bias);
+  r->bias_vals.assign(pen->bias_values, pen->bias_values + pen->n_bias);
+  r->penalized = r->freq_pen != 0.f || r->pres_pen != 0.f || pen->n_bias != 0;
+  return LLMLB_OK;
+}
+
 extern "C" int llmlb_request_submit(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt,
                                     const llmlb_sampling* s, uint64_t* req_id) {
-  if (!e || !prompt_ids || !s || !req_id || n_prompt == 0) { set_error("llmlb_request_submit: bad argument"); return LLMLB_E_INVALID_ARG; }
+  return llmlb_request_submit_penalized(e, prompt_ids, n_prompt, s, nullptr, req_id);
+}
+
+extern "C" int llmlb_request_submit_penalized(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt,
+                                              const llmlb_sampling* s, const llmlb_penalties* pen, uint64_t* req_id) {
+  if (!e || !prompt_ids || !s || !req_id || n_prompt == 0) {
+    set_error(pen ? "llmlb_request_submit_penalized: bad argument" : "llmlb_request_submit: bad argument");
+    return LLMLB_E_INVALID_ARG;
+  }
   if (s->max_tokens == 0) { set_error("max_tokens must be > 0"); return LLMLB_E_INVALID_ARG; }
   if (uint64_t(n_prompt) + s->max_tokens > e->cfg.max_ctx) {
     set_error("prompt + max_tokens exceeds the context length");
@@ -1611,6 +1714,7 @@ extern "C" int llmlb_request_submit(llmlb_engine* e, const int32_t* prompt_ids, 
     if (prompt_ids[i] < 0 || uint32_t(prompt_ids[i]) >= e->M.vocab) { set_error("token id out of range"); return LLMLB_E_INVALID_ARG; }
   if (s->temperature < 0.f || s->top_p < 0.f) { set_error("negative temperature/top_p"); return LLMLB_E_INVALID_ARG; }
   auto r = std::make_shared<Request>();
+  RC(take_penalties(pen, e->M.vocab, r.get()));
   r->prompt.assign(prompt_ids, prompt_ids + n_prompt);
   r->n_prompt0 = n_prompt;
   r->s = *s;
@@ -1627,8 +1731,10 @@ extern "C" int llmlb_request_submit(llmlb_engine* e, const int32_t* prompt_ids, 
     e->requests[r->id] = r;
     e->waiting.push_back(r);
     *req_id = r->id;
-    if (e->plan_on) {   // id, sampling, prompt and stop ids travel to the followers in queue order
-      std::vector<uint8_t> rec(8 + sizeof(llmlb_sampling) + 8 + (size_t(n_prompt) + r->stop_ids.size()) * 4);
+    if (e->plan_on) {   // id, sampling, prompt, stop ids and (penalised requests) the penalties travel to the followers in queue order
+      const uint32_t n_bias = uint32_t(r->bias_ids.size());
+      std::vector<uint8_t> rec(8 + sizeof(llmlb_sampling) + 8 + (size_t(n_prompt) + r->stop_ids.size()) * 4 +
+                               (r->penalized ? 12 + size_t(n_bias) * 8 : 0));
       uint8_t* p = rec.data();
       memcpy(p, &r->id, 8); p += 8;
       memcpy(p, &r->s, sizeof(llmlb_sampling)); p += sizeof(llmlb_sampling);
@@ -1636,6 +1742,11 @@ extern "C" int llmlb_request_submit(llmlb_engine* e, const int32_t* prompt_ids, 
       memcpy(p, &n_prompt, 4); memcpy(p + 4, &n_stop, 4); p += 8;
       memcpy(p, r->prompt.data(), size_t(n_prompt) * 4); p += size_t(n_prompt) * 4;
       if (n_stop) memcpy(p, r->stop_ids.data(), size_t(n_stop) * 4);
+      p += size_t(n_stop) * 4;
+      if (r->penalized) {   // [f32 frequency][f32 presence][u32 n_bias][i32 ids][f32 values]
+        memcpy(p, &r->freq_pen, 4); memcpy(p + 4, &r->pres_pen, 4); memcpy(p + 8, &n_bias, 4); p += 12;
+        if (n_bias) { memcpy(p, r->bias_ids.data(), size_t(n_bias) * 4); memcpy(p + size_t(n_bias) * 4, r->bias_vals.data(), size_t(n_bias) * 4); }
+      }
       e->plan_log(kPlanSubmit, rec.data(), uint32_t(rec.size()));
     }
   }

@@ -55,6 +55,11 @@ class Sampling(C.Structure):
                 ("n_stop_ids", C.c_uint32), ("ignore_eos", C.c_uint32)]
 
 
+class Penalties(C.Structure):
+    _fields_ = [("frequency_penalty", C.c_float), ("presence_penalty", C.c_float),
+                ("bias_ids", C.POINTER(C.c_int32)), ("bias_values", C.POINTER(C.c_float)), ("n_bias", C.c_uint32)]
+
+
 class TokenEvent(C.Structure):
     _fields_ = [("token_id", C.c_int32), ("index", C.c_uint32), ("finish_reason", C.c_uint32),
                 ("prompt_tokens", C.c_uint32), ("completion_tokens", C.c_uint32),
@@ -78,6 +83,7 @@ PROTOTYPES = {
     "llmlb_engine_health": (C.c_int, [vp, _P(Health)]),
     "llmlb_engine_pause": (C.c_int, [vp, u32]),
     "llmlb_request_submit": (C.c_int, [vp, _P(i32), u32, _P(Sampling), _P(u64)]),
+    "llmlb_request_submit_penalized": (C.c_int, [vp, _P(i32), u32, _P(Sampling), _P(Penalties), _P(u64)]),
     "llmlb_request_poll": (C.c_int, [vp, u64, _P(TokenEvent), u32, _P(u32), C.c_int]),
     "llmlb_request_cancel": (C.c_int, [vp, u64]),
     "llmlb_request_release": (C.c_int, [vp, u64]),
@@ -101,6 +107,7 @@ PROTOTYPES = {
     "llmlb_op_decode_attention": (C.c_int, [vp, vp, vp, vp, u32, vp, vp, u32, vp, u32, u32, vp,
                                             u32, u32, vp, vp]),
     "llmlb_op_sample": (C.c_int, [vp, u32, u32, vp, vp, vp, vp, vp, vp, vp]),
+    "llmlb_op_penalize": (C.c_int, [vp, u32, u32, vp, u64, vp, vp, vp, vp, vp, u32, vp]),
     "llmlb_op_allreduce": (C.c_int, [vp, vp, u64, vp]),
     "llmlb_op_synth_bf16": (C.c_int, [vp, u64, u64, u64, u64, u64, u64, u32, f32, vp]),
 }
@@ -211,7 +218,10 @@ class Engine:
 
     # ---- requests ----
     def submit(self, prompt_ids, max_tokens, temperature=0.0, top_k=0, top_p=1.0, seed=0,
-               stop_ids=(), ignore_eos=False):
+               stop_ids=(), ignore_eos=False, frequency_penalty=None, presence_penalty=None, logit_bias=None):
+        """frequency_penalty / presence_penalty / logit_bias ({token id: value}): OpenAI's penalties, applied on the device
+        before sampling (llmlb_penalties).  Given at all (even neutral), the request goes through
+        llmlb_request_submit_penalized."""
         n = len(prompt_ids)
         arr = (i32 * n)(*prompt_ids)
         s = Sampling()
@@ -221,7 +231,17 @@ class Engine:
         s.n_stop_ids = len(stop_ids)
         s.ignore_eos = 1 if ignore_eos else 0
         rid = u64()
-        check(lib().llmlb_request_submit(self._h, arr, n, C.byref(s), C.byref(rid)))
+        if frequency_penalty is None and presence_penalty is None and logit_bias is None:
+            check(lib().llmlb_request_submit(self._h, arr, n, C.byref(s), C.byref(rid)))
+            return rid.value
+        bias = list((logit_bias or {}).items())
+        ids = (i32 * max(1, len(bias)))(*[int(k) for k, _ in bias])
+        vals = (f32 * max(1, len(bias)))(*[float(v) for _, v in bias])
+        pen = Penalties()
+        pen.frequency_penalty = frequency_penalty or 0.0
+        pen.presence_penalty = presence_penalty or 0.0
+        pen.bias_ids, pen.bias_values, pen.n_bias = C.cast(ids, _P(i32)), C.cast(vals, _P(f32)), len(bias)
+        check(lib().llmlb_request_submit_penalized(self._h, arr, n, C.byref(s), C.byref(pen), C.byref(rid)))
         return rid.value
 
     def poll(self, rid, cap=256, timeout_ms=0):

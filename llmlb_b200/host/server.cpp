@@ -22,6 +22,7 @@
 #include <cerrno>
 #include <chrono>
 #include <climits>
+#include <cmath>
 #include <cstring>
 #include <fstream>
 #include <map>
@@ -36,6 +37,7 @@
 // engine library of the same ABI version that predates it (and refuses a scaled checkpoint there instead of serving it
 // unscaled), such as the scripted engine the CPU tests link it against.
 #pragma weak llmlb_engine_set_rope_freq_factors
+#pragma weak llmlb_request_submit_penalized
 #include "anthropic.hpp"
 #include "checkpoint.hpp"
 #include "download.hpp"
@@ -308,6 +310,58 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
     else if (sp->is_array()) for (auto& x : sp->items()) if (x.is_string()) stop_strings.push_back(x.str());
   }
   StopMatcher stopper(stop_strings);
+  // OpenAI's frequency_penalty, presence_penalty and logit_bias (chat and completions): null or absent is the default, and
+  // a value the engine cannot serve is refused rather than dropped
+  llmlb_penalties pen{};
+  std::vector<int32_t> bias_ids;
+  std::vector<float> bias_vals;
+  if (kind != 1 && !anthropic) {
+    for (const char* k : {"frequency_penalty", "presence_penalty"}) {
+      const Json* v = req.get(k);
+      if (!v || v->is_null()) continue;
+      const double d = v->as_double();
+      if (!v->is_number() || !std::isfinite(d) || d < -2.0 || d > 2.0) {
+        send_err(400, std::string(k) + " must be a number in [-2, 2]", "invalid_request_error");
+        return;
+      }
+      (k[0] == 'f' ? pen.frequency_penalty : pen.presence_penalty) = float(d);
+    }
+    const Json* lb = req.get("logit_bias");
+    if (lb && !lb->is_null()) {
+      if (!lb->is_object()) { send_err(400, "logit_bias must be an object mapping token ids to numbers", "invalid_request_error"); return; }
+      if (lb->members().size() > LLMLB_MAX_LOGIT_BIAS) { send_err(400, "logit_bias has more than 1024 entries", "invalid_request_error"); return; }
+      for (auto& kv : lb->members()) {
+        const std::string& key = kv.first;
+        const bool digits = !key.empty() && key.size() <= 10 && key.find_first_not_of("0123456789") == std::string::npos;
+        const uint64_t id = digits ? strtoull(key.c_str(), nullptr, 10) : 0;
+        if (!digits || id >= G.vocab) {
+          send_err(400, "logit_bias: key '" + key + "' is not a token id of the vocabulary (a decimal integer below " + std::to_string(G.vocab) + ")",
+                   "invalid_request_error");
+          return;
+        }
+        const double d = kv.second.as_double();
+        if (!kv.second.is_number() || !std::isfinite(d) || d < -100.0 || d > 100.0) {
+          send_err(400, "logit_bias: the value for token " + key + " must be a number in [-100, 100]", "invalid_request_error");
+          return;
+        }
+        if (std::find(bias_ids.begin(), bias_ids.end(), int32_t(id)) != bias_ids.end()) {
+          send_err(400, "logit_bias: token " + std::to_string(id) + " appears twice", "invalid_request_error");
+          return;
+        }
+        bias_ids.push_back(int32_t(id));
+        bias_vals.push_back(float(d));
+      }
+    }
+  }
+  const bool penalized = pen.frequency_penalty != 0.f || pen.presence_penalty != 0.f || !bias_ids.empty();
+  if (penalized && !llmlb_request_submit_penalized) {
+    send_err(400, "frequency_penalty, presence_penalty and logit_bias are not supported by the engine library this server runs on",
+             "invalid_request_error");
+    return;
+  }
+  pen.bias_ids = bias_ids.data();
+  pen.bias_values = bias_vals.data();
+  pen.n_bias = uint32_t(bias_ids.size());
   const bool stream = req.get("stream") && req.get("stream")->as_bool();
   bool include_usage = kind == 1;
   if (const Json* so = req.get("stream_options")) if (const Json* iu = so->get("include_usage")) include_usage = iu->as_bool();
@@ -315,7 +369,9 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
 
   const auto t0 = std::chrono::steady_clock::now();
   uint64_t rid = 0;
-  int rc = s.max_tokens ? llmlb_request_submit(G.eng, ids.data(), uint32_t(ids.size()), &s, &rid) : LLMLB_E_INVALID_ARG;
+  int rc = !s.max_tokens ? LLMLB_E_INVALID_ARG
+           : penalized    ? llmlb_request_submit_penalized(G.eng, ids.data(), uint32_t(ids.size()), &s, &pen, &rid)
+                          : llmlb_request_submit(G.eng, ids.data(), uint32_t(ids.size()), &s, &rid);
   if (rc == LLMLB_E_QUEUE_FULL) {   // openai.rs:841-861: 429 rate_limit_exceeded + Retry-After = queue timeout
     const ClientError qe = queue_capacity_exceeded(G.queue_timeout_ms / 1000);
     const std::string ra = "Retry-After: " + std::to_string(qe.retry_after) + "\r\n";
