@@ -160,7 +160,7 @@ typedef struct llmlb_sampling {
   uint32_t max_tokens;             /* generated-token budget (max_tokens / max_output_tokens) */
   float temperature;               /* 0 = greedy arg-max */
   uint32_t top_k;                  /* 0 = off */
-  float top_p;                     /* >=1 or 0 = off */
+  float top_p;                     /* >=1 = off; 0 keeps only the most probable token(s) */
   uint64_t seed;                   /* per-request RNG stream */
   const int32_t* stop_ids;         /* optional stop / EOS token ids */
   uint32_t n_stop_ids;

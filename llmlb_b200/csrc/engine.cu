@@ -12,6 +12,7 @@
 
 #include <algorithm>
 #include <chrono>
+#include <cmath>
 #include <condition_variable>
 #include <cstdlib>
 #include <cstring>
@@ -1713,6 +1714,7 @@ extern "C" int llmlb_request_submit_penalized(llmlb_engine* e, const int32_t* pr
   for (uint32_t i = 0; i < n_prompt; ++i)
     if (prompt_ids[i] < 0 || uint32_t(prompt_ids[i]) >= e->M.vocab) { set_error("token id out of range"); return LLMLB_E_INVALID_ARG; }
   if (s->temperature < 0.f || s->top_p < 0.f) { set_error("negative temperature/top_p"); return LLMLB_E_INVALID_ARG; }
+  if (std::isnan(s->temperature) || std::isnan(s->top_p)) { set_error("temperature/top_p is NaN"); return LLMLB_E_INVALID_ARG; }
   auto r = std::make_shared<Request>();
   RC(take_penalties(pen, e->M.vocab, r.get()));
   r->prompt.assign(prompt_ids, prompt_ids + n_prompt);

@@ -2,10 +2,13 @@
 //
 // One CTA (1024 threads) per row of fp32 logits [vocab].  Definition (mirrored by
 // oracle/sampling_ref.py):
-//   z_i = logit_i / T, e_i = exp(z_i - max z)
+//   T <= 0 (or NaN): arg-max, lowest index on ties
+//   e_i = exp((logit_i - max logit) / T)                      (the max maps to exactly 1: no finite
+//                                                               T > 0 overflows into inf - inf)
 //   top-k : keep e_i >= (k-th largest e)                      (ties at the threshold all kept)
-//   top-p : of those, keep e_i >= v where v is the value at which the descending cumulative
-//           mass first reaches top_p * (kept mass)            (ties kept)
+//   top-p : for top_p < 1, of those keep e_i >= v where v is the value at which the descending
+//           cumulative mass first reaches top_p * (kept mass) (ties kept; top_p <= 0 keeps the
+//           maximum(s))
 //   draw  : u = U[0,1) from (seed, step); the first index in VOCAB order whose running kept
 //           mass exceeds u * (kept mass)
 // Thresholds are found by an 8-bit radix select over the (monotone) bit pattern of e_i: each
@@ -15,6 +18,8 @@
 // associative, so the threshold — and with it the sampled token — does not depend on the order in
 // which threads reach the atomics.  Tensor-parallel ranks sample the same all-gathered logits
 // independently and must agree bit for bit (their schedulers replay each other's finishes).
+// The draw sums e in fp32 in a fixed order (no atomics), and always resolves to a kept token
+// with e > 0 inside the warp span that holds the target (see the search below).
 #include "../../include/llmlb_b200.h"
 #include "common.cuh"
 
@@ -23,6 +28,13 @@ namespace llmlb {
 constexpr int kSampThreads = 1024;
 typedef unsigned long long u64q;   // probability mass in units of 2^-40 (e <= 1, vocab < 2^17: sums stay below 2^58)
 __device__ __forceinline__ u64q mass_q(float e) { return (u64q)__float2ull_rd(e * 1099511627776.f); }
+
+// e = exp((logit - lmax) / T).  The max maps to exp(0) = 1 and everything below it to a finite or
+// -inf exponent, even when 1/T overflows to inf (T below ~3e-39): (0 * inf) is never formed.
+__device__ __forceinline__ float scaled_exp(float logit, float lmax, float inv_t) {
+  const float d = logit - lmax;
+  return __expf(d < 0.f ? d * inv_t : 0.f);
+}
 
 __device__ __forceinline__ float block_reduce_max(float v, float* red) {
   v = warp_max(v);
@@ -47,7 +59,7 @@ __device__ __forceinline__ float block_reduce_sum(float v, float* red) {
 // mode 0: largest key v such that count(e >= v) >= target_count
 // mode 1: largest key v such that mass(e >= v)  >= target_mass
 __device__ uint32_t radix_select(const float* __restrict__ logits, uint32_t vocab, float inv_t,
-                                 float zmax, uint32_t floor_key, int mode, uint32_t target_count,
+                                 float lmax, uint32_t floor_key, int mode, uint32_t target_count,
                                  u64q target_mass, int* s_cnt, u64q* s_mass, uint32_t* s_sel,
                                  u64q* s_above) {
   uint32_t prefix = 0, prefix_mask = 0;
@@ -60,7 +72,7 @@ __device__ uint32_t radix_select(const float* __restrict__ logits, uint32_t voca
     }
     __syncthreads();
     for (uint32_t i = threadIdx.x; i < vocab; i += kSampThreads) {
-      float e = __expf((logits[i] * inv_t) - zmax);
+      float e = scaled_exp(logits[i], lmax, inv_t);
       uint32_t key = __float_as_uint(e);
       if (key >= floor_key && (key & prefix_mask) == prefix) {
         uint32_t b = (key >> shift) & 255u;
@@ -170,7 +182,7 @@ sample_kernel(const float* __restrict__ logits_all, uint32_t vocab,
   const float T = temperature ? temperature[row] : 0.f;
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 
-  if (T <= 0.f) {  // greedy: max value, lowest index on ties
+  if (!(T > 0.f)) {  // greedy: max value, lowest index on ties
     float best = -INFINITY;
     int bi = 0x7fffffff;
     for (uint32_t i = threadIdx.x; i < vocab; i += kSampThreads) {
@@ -200,20 +212,20 @@ sample_kernel(const float* __restrict__ logits_all, uint32_t vocab,
   }
 
   const float inv_t = 1.f / T;
-  float zm = -INFINITY;
-  for (uint32_t i = threadIdx.x; i < vocab; i += kSampThreads) zm = fmaxf(zm, logits[i] * inv_t);
-  zm = block_reduce_max(zm, red);
+  float lmax = -INFINITY;
+  for (uint32_t i = threadIdx.x; i < vocab; i += kSampThreads) lmax = fmaxf(lmax, logits[i]);
+  lmax = block_reduce_max(lmax, red);
 
   uint32_t floor_key = 0;
   const int32_t k = top_k ? top_k[row] : 0;
   if (k > 0 && uint32_t(k) < vocab)
-    floor_key = radix_select(logits, vocab, inv_t, zm, 0u, 0, uint32_t(k), 0ull, s_cnt, s_mass,
+    floor_key = radix_select(logits, vocab, inv_t, lmax, 0u, 0, uint32_t(k), 0ull, s_cnt, s_mass,
                              s_sel, s_above);
   const float p = top_p ? top_p[row] : 1.f;
-  if (p > 0.f && p < 1.f) {
+  if (p < 1.f) {   // top_p <= 0: a target mass of 0 selects the largest key, the maximum(s)
     u64q mass = 0;   // kept mass, same fixed point as the bins (integer sums: order-free)
     for (uint32_t i = threadIdx.x; i < vocab; i += kSampThreads) {
-      float e = __expf(logits[i] * inv_t - zm);
+      float e = scaled_exp(logits[i], lmax, inv_t);
       if (__float_as_uint(e) >= floor_key) mass += mass_q(e);
     }
 #pragma unroll
@@ -224,7 +236,7 @@ sample_kernel(const float* __restrict__ logits_all, uint32_t vocab,
     for (int w = 0; w < 32; ++w) mass += red_q[w];
     __syncthreads();
     const u64q target_q = (u64q)__double2ull_rd(double(p) * double(mass));
-    floor_key = radix_select(logits, vocab, inv_t, zm, floor_key, 1, 0u, target_q, s_cnt, s_mass,
+    floor_key = radix_select(logits, vocab, inv_t, lmax, floor_key, 1, 0u, target_q, s_cnt, s_mass,
                              s_sel, s_above);
   }
 
@@ -233,7 +245,7 @@ sample_kernel(const float* __restrict__ logits_all, uint32_t vocab,
   const uint32_t w0 = warp * span;
   float wsum = 0.f;
   for (uint32_t i = w0 + lane; i < min(vocab, w0 + span); i += 32) {
-    float e = __expf(logits[i] * inv_t - zm);
+    float e = scaled_exp(logits[i], lmax, inv_t);
     if (__float_as_uint(e) >= floor_key) wsum += e;
   }
   wsum = warp_sum(wsum);
@@ -250,14 +262,21 @@ sample_kernel(const float* __restrict__ logits_all, uint32_t vocab,
   uint64_t h = mix64(mix64(seed ? seed[row] : 0ull) + (step ? step[row] : 0ull));
   const float u = float(uint32_t(h >> 40)) * (1.0f / 16777216.0f);
   const float target = u * total;
-  // exactly one warp holds the crossing (before <= target < before + wsum)
+  // The warp intervals [before, before + wsum) tile [0, total) exactly: every thread forms `before`
+  // and `total` by the same fp32 chain over s_warp_tot, and target = fl(u * total) < total for
+  // u <= 1 - 2^-24.  So exactly one warp holds the target whenever total is finite.
   if (target >= before && target < before + wsum) {
+    // The search below adds the same e in a different fp32 order (row scans, carried across rows)
+    // than the lane sums and butterfly that formed wsum; the two totals differ by a few ulps.  A
+    // target in between crosses no lane: it then belongs to this span's last kept token with e > 0
+    // (one exists, since wsum > 0), whose CDF end is within that rounding of the target.
     float run = before;
+    int found = -1, last = -1;
     for (uint32_t base = w0; base < min(vocab, w0 + span); base += 32) {
       uint32_t i = base + lane;
       float e = 0.f;
       if (i < vocab) {
-        float ee = __expf(logits[i] * inv_t - zm);
+        float ee = scaled_exp(logits[i], lmax, inv_t);
         if (__float_as_uint(ee) >= floor_key) e = ee;
       }
       float inc = e;
@@ -268,32 +287,18 @@ sample_kernel(const float* __restrict__ logits_all, uint32_t vocab,
       }
       uint32_t hit = __ballot_sync(0xffffffffu, e > 0.f && run + inc > target);
       if (hit) {
-        if (lane == 0) s_result = int(base + (__ffs(hit) - 1));
+        found = int(base + (__ffs(hit) - 1));
         break;
       }
+      uint32_t pos = __ballot_sync(0xffffffffu, e > 0.f);
+      if (pos) last = int(base + (31 - __clz(pos)));
       run += __shfl_sync(0xffffffffu, inc, 31);
     }
+    if (lane == 0) s_result = found >= 0 ? found : last;
   }
   __syncthreads();
-  if (s_result < 0) {
-    // numerical corner (target == total): last kept index
-    int last = -1;
-    for (uint32_t i = threadIdx.x; i < vocab; i += kSampThreads) {
-      float e = __expf(logits[i] * inv_t - zm);
-      if (__float_as_uint(e) >= floor_key) last = int(i);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) last = max(last, __shfl_xor_sync(0xffffffffu, last, o));
-    if (lane == 0) red_i[warp] = last;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      int l = -1;
-      for (int w = 0; w < 32; ++w) l = max(l, red_i[w]);
-      s_result = l < 0 ? 0 : l;
-    }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) out_ids[row] = s_result;
+  // s_result < 0 only when no warp holds the target: NaN or infinite logits (total not finite)
+  if (threadIdx.x == 0) out_ids[row] = s_result < 0 ? 0 : s_result;
 }
 
 }  // namespace llmlb

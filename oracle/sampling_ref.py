@@ -16,13 +16,17 @@ def uniform(seed, step):
 
 
 def kept_mask(logits, temperature, top_k, top_p):
-    z = logits.astype(np.float32) * np.float32(1.0 / np.float32(temperature))
-    e = np.exp((z - z.max()).astype(np.float32)).astype(np.float32)
+    lg = logits.astype(np.float32)
+    d = lg - lg.max()
+    with np.errstate(over="ignore", invalid="ignore"):
+        inv_t = np.float32(1.0) / np.float32(temperature)      # inf below T ~ 3e-39: the max still maps to 0
+        z = np.where(d < 0, d * inv_t, np.float32(0)).astype(np.float32)
+    e = np.exp(z).astype(np.float32)
     keep = np.ones_like(e, dtype=bool)
     if 0 < top_k < e.size:
         kth = np.sort(e)[::-1][top_k - 1]
         keep &= e >= kth
-    if 0.0 < top_p < 1.0:
+    if top_p < 1.0:                          # top_p <= 0: target 0, the maximum(s) alone
         ek = np.where(keep, e, 0).astype(np.float64)
         order = np.argsort(-ek, kind="stable")
         cs = np.cumsum(ek[order])
@@ -37,7 +41,7 @@ def kept_mask(logits, temperature, top_k, top_p):
 def sample(logits, temperature, top_k, top_p, seed, step):
     """Returns (token, margin): margin = relative distance of the draw from the nearest CDF
     edge; tiny margins mark draws where fp32 summation order may legitimately flip the answer."""
-    if temperature <= 0:
+    if not temperature > 0:
         return int(np.argmax(logits)), 1.0
     e, keep = kept_mask(logits, temperature, top_k, top_p)
     ek = np.where(keep, e, 0).astype(np.float64)

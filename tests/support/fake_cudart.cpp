@@ -213,7 +213,8 @@ cudaError_t cudaGraphExecDestroy(cudaGraphExec_t x) { free(x); return cudaSucces
 // tests/test_kernel_coverage_cpu.py can tell a K-split launch from a plain one.  Launches of the K-split decode GEMV
 // (gemv_ks_kernel, whose 9th parameter is TW, the warps of a team) append TW, which sets the kernel's team count.  The
 // residual fold (rmsnorm_parts_kernel / rmsnorm_parts_cluster_kernel) appends n_parts, whether a gain was given (0 / 1)
-// and hidden; rope_append_kernel appends n_heads and n_kv; rmsnorm_kernel and embed_kernel append hidden.
+// and hidden; rope_append_kernel appends n_heads and n_kv; rmsnorm_kernel and embed_kernel append hidden; sample_kernel
+// appends vocab.
 static void log_launch(const void* fn, dim3 g, dim3 b, size_t smem, dim3 cluster, int pdl, void** args = nullptr) {
   static FILE* f = getenv("FAKE_CUDART_LAUNCH_LOG") ? fopen(getenv("FAKE_CUDART_LAUNCH_LOG"), "a") : nullptr;
   if (!f) return;
@@ -228,6 +229,7 @@ static void log_launch(const void* fn, dim3 g, dim3 b, size_t smem, dim3 cluster
     fprintf(f, " %u %d %u", u32(2), *static_cast<void* const*>(args[4]) != nullptr, u32(6));
   if (args && strstr(name, "18rope_append_kernel")) fprintf(f, " %u %u", u32(6), u32(7));
   if (args && (strstr(name, "14rmsnorm_kernel") || strstr(name, "12embed_kernel"))) fprintf(f, " %u", u32(3));
+  if (args && strstr(name, "13sample_kernel")) fprintf(f, " %u", u32(1));     // (logits, vocab, ...)
   fputc('\n', f);
   fflush(f);
 }

@@ -1,13 +1,15 @@
 """The launches of the GPU kernel tests (tests/test_kernels_sm90_gpu.py, tests/test_gemv_sm90_gpu.py,
 tests/test_step_kernels_sm90_gpu.py), made over the fake CUDA runtime with FAKE_CUDART_LAUNCH_LOG set: every GEMM case through
 the entry point it uses there, the wave-tail pair, every decode split, both prefill attention kernels, every GEMV case through
-llmlb_op_gemv, and the residual fold, RMSNorm, RoPE / KV-append and embedding cases.  Nothing executes; the log is the launch
+llmlb_op_gemv, the residual fold, RMSNorm, RoPE / KV-append and embedding cases, and the sampler's vocabularies
+(tests/test_sampling_sm90_gpu.py).  Nothing executes; the log is the launch
 plan of the test cases.  Every section is optional.
 usage: kernel_case_sweep.py <cases.json>   ({"gemm": [[T, n_out, K, epi], ...], "wave_tail": [T, n_out, K, main_rows],
                                              "decode_splits": [...], "max_split": n,
                                              "gemv": [[n_out, K, tokens, epi, norm, out_stride], ...],
                                              "fold": [[T, H, n_parts, gain, part_stride], ...], "rmsnorm": [[T, H], ...],
-                                             "rope": [[T, n_heads, n_kv], ...], "embed": [[T, H, vocab], ...]})"""
+                                             "rope": [[T, n_heads, n_kv], ...], "embed": [[T, H, vocab], ...],
+                                             "sample": [[rows, vocab], ...]})"""
 import ctypes
 import json
 import os
@@ -75,3 +77,6 @@ for T, nh, nkv in cases.get("rope", []):
 for T, H, V in cases.get("embed", []):
     mark("embed %d %d" % (T, H))
     ffi.check(L.llmlb_op_embed(w, x, out, T, H, V, None))
+for R, V in cases.get("sample", []):
+    mark("sample %d %d" % (R, V))
+    ffi.check(L.llmlb_op_sample(w, R, V, x, x, x, x, x, out, None))

@@ -134,6 +134,23 @@ def test_scenario_stop_ids_cancel_release_and_argument_checks():
 
 
 @inner
+def test_scenario_nan_temperature_or_top_p_is_refused_at_submit():
+    """NaN < 0 is false, so a range check alone lets NaN through to the sampler; submit names it instead."""
+    ffi = _ffi()
+    nan = float("nan")
+    with ffi.Engine(TINY, max_seqs=2, max_ctx=256) as eng:
+        for kw in (dict(temperature=nan), dict(top_p=nan), dict(temperature=nan, top_p=nan), dict(temperature=0.7, top_p=nan),
+                   dict(temperature=nan, frequency_penalty=0.5)):
+            with pytest.raises(ffi.LlmlbError, match="NaN"):
+                eng.submit([1, 2, 3], 4, **kw)
+        # the edges that stay legal: 0, the smallest positive temperature, top_p 0 and 1
+        for kw in (dict(temperature=0.0), dict(temperature=1.4e-45), dict(temperature=0.5, top_p=0.0), dict(temperature=0.5, top_p=1.0)):
+            evs = drain(eng, eng.submit([1, 2, 3], 2, ignore_eos=True, **kw))
+            assert evs[-1]["finish_reason"] == LENGTH
+        assert settle(eng)["free_kv_pages"] == eng.health()["total_kv_pages"]
+
+
+@inner
 def test_scenario_oversubscribed_pages_preempt_and_everything_still_completes():
     """kv_pages far below what the running set needs: sequences take pages as they grow, the youngest is evicted when the
     pool runs dry and recomputed later; every request still delivers exactly max_tokens events, in order, once."""

@@ -21,6 +21,10 @@ would notice the mistakes they are meant to catch.
     launched by a GPU kernel test case or listed with the test that covers it; and the fold, norm and RoPE checkers reject
     a dropped or reordered part, a gain a quarter off, a missing DSMEM exchange, another token's RMS scale, wrong RoPE
     pairs, positions or sin sign, and K in the neighbouring page slot.
+  * sampler (tests/test_sampling_sm90_gpu.py): its vocabularies cover every vocabulary the engine samples at 8B, MID and
+    70B; and its draw checker, applied to a numpy model of the kernel's fp32 orders, rejects the old fallback to the last
+    kept index on draws inside the gap between the warp totals and the row scans, a run not carried across rows, a strict
+    top-k threshold, top-p one token short, u from step + 1, and top_p = 0 taken as "off".
 """
 import collections
 import json
@@ -30,6 +34,7 @@ import re
 import subprocess
 import sys
 
+import numpy as np
 import pytest
 import torch
 
@@ -38,6 +43,7 @@ sys.path.insert(0, HERE)
 import test_engine_host_logic_cpu as HL  # noqa: E402
 import test_gemv_sm90_gpu as GV  # noqa: E402
 import test_kernels_sm90_gpu as K  # noqa: E402
+import test_sampling_sm90_gpu as SS  # noqa: E402
 import test_step_kernels_sm90_gpu as SK  # noqa: E402
 
 GEMM_RE = re.compile(r"(gemm_tc2?_kernel)ILi(\d+)ELi(\d+)E")
@@ -60,7 +66,7 @@ def classes(log):
     ("decode", cluster size) for decode attention (1 = the unsplit tensor-core kernel), ("prefill", kernel),
     ("gemv_ks", B, EPI, NORM, CW, TW) for the K-split GEMV, ("gemv", B, EPI, NORM) for the row-owner GEMV,
     ("fold", kernel, n_parts, gain, H) for the residual fold, ("rope", n_heads, n_kv), ("rmsnorm_kernel", H) and
-    ("embed_kernel", H)."""
+    ("embed_kernel", H) and ("sample", vocab)."""
     out, ctx = collections.defaultdict(set), "init"
     for line in open(log):
         if line.startswith("###"):
@@ -75,6 +81,10 @@ def classes(log):
         if name == "rope_append_kernel":
             assert len(p) == 14, line            # n_heads, n_kv appended
             out[ctx].add(("rope", int(p[12]), int(p[13])))
+            continue
+        if name == "sample_kernel":
+            assert len(p) == 13, line            # vocab appended
+            out[ctx].add(("sample", int(p[12])))
             continue
         if name in ("rmsnorm_kernel", "embed_kernel"):
             assert len(p) == 13, line            # hidden appended
@@ -505,7 +515,6 @@ def test_gemv_probe_rejects_a_gain_shifted_by_8(epi):
 # test_every_kernel_of_the_launch_plans_is_gpu_tested_or_classified.
 COVERED_ELSEWHERE = {
     "rope_table_kernel": "test_rope_scaling_gpu.py (the scaled table against fp64 up to position 131071)",
-    "sample_kernel": "test_ops_gpu.py (sampling against oracle.sampling_ref)",
     "slot_init_kernel": "the engine tests (test_engine_gpu.py, test_parity_8b_gpu.py): step bookkeeping",
     "prefill_finish_kernel": "the engine tests: step bookkeeping",
     "step_finish_kernel": "the engine tests: step bookkeeping",
@@ -528,6 +537,12 @@ def _step_case_plan(tmp_path):
         "rope": [[T, nh, nkv] for nh, nkv in SK.ROPE_HEADS for T in SK.ROPE_TOKENS],
         "embed": [[T, H, SK.EMBED_VOCAB] for T, H in SK.EMBED_CASES]}))
     return run_logged(tmp_path, "step_cases", [os.path.join(HERE, "support", "kernel_case_sweep.py"), str(spec)])
+
+
+def _sample_case_plan(tmp_path):
+    spec = tmp_path / "sample_cases.json"
+    spec.write_text(json.dumps({"sample": [[3, V] for V in SS.VOCABS]}))
+    return run_logged(tmp_path, "sample_cases", [os.path.join(HERE, "support", "kernel_case_sweep.py"), str(spec)])
 
 
 def _engine_plan(tmp_path, model, tp, max_width=None, parse=classes):
@@ -584,7 +599,7 @@ def test_gpu_step_kernel_cases_launch_every_class_the_engine_launches(built_lib,
 
 def test_every_kernel_of_the_launch_plans_is_gpu_tested_or_classified(built_lib, tmp_path):
     """Every kernel the tp = 1 engine launches (8B, LLAMA_MID, 70B) is launched by a GPU kernel test case (GEMMs,
-    attention, GEMVs, step kernels) or is listed in COVERED_ELSEWHERE with the test that covers it.  A kernel added to
+    attention, GEMVs, step kernels, sampler) or is listed in COVERED_ELSEWHERE with the test that covers it.  A kernel added to
     the engine fails here until someone classifies it."""
     cases = {"gemm": [[T, N, Kd, e] for T, N, Kd, epis in K.GEMM_CASES for e in epis],
              "wave_tail": list(K.WAVE_TAIL_CASE) + [K.wave_tail_rows(*K.WAVE_TAIL_CASE[:2])],
@@ -594,7 +609,8 @@ def test_every_kernel_of_the_launch_plans_is_gpu_tested_or_classified(built_lib,
     run_logged(tmp_path, "cases", [os.path.join(HERE, "support", "kernel_case_sweep.py"), str(spec)])
     _gemv_sweep(tmp_path, "gemv_cases", GV.gemv_params())
     _step_case_plan(tmp_path)
-    tested = set().union(*(launched_kernels(tmp_path, n) for n in ("cases", "gemv_cases", "step_cases")))
+    _sample_case_plan(tmp_path)
+    tested = set().union(*(launched_kernels(tmp_path, n) for n in ("cases", "gemv_cases", "step_cases", "sample_cases")))
     engine = set()
     for model in PLAN_MODELS:
         _engine_plan(tmp_path, model, 1)
@@ -719,3 +735,109 @@ def test_rope_checker_rejects_wrong_pairs_positions_sin_sign_and_slot():
     assert _rope_rejects(pos_shift=-1) > 0
     assert _rope_rejects(sin_sign=-1.0) > 0
     assert _rope_rejects(slot_shift=1) > 0
+
+
+# ------------------------------------------------------------------------------------------------------------- sampler --
+def _sample_classes(per_ctx):
+    return {c for cs in per_ctx.values() for c in cs if c[0] == "sample"}
+
+
+def test_gpu_sampler_cases_launch_every_vocab_the_engine_launches(built_lib, tmp_path):
+    """Every vocabulary the tp = 1 engine samples at Llama-3-8B, LLAMA_MID and Llama-3-70B shapes is among the
+    vocabularies tests/test_sampling_sm90_gpu.py launches sample_kernel with."""
+    tested = _sample_classes(_sample_case_plan(tmp_path))
+    assert tested == {("sample", V) for V in SS.VOCABS}, sorted(tested)
+    assert any(V % 32 for V in SS.VOCABS)
+    engine = {}
+    for model in PLAN_MODELS:
+        for c in _sample_classes(_engine_plan(tmp_path, model, 1, 8)):
+            engine.setdefault(c, model)
+    assert {c[1] for c in engine} >= {128256, 4096}, sorted(engine)
+    missing = sorted((c, model) for c, model in engine.items() if c not in tested)
+    assert not missing, "the engine samples vocabularies no GPU sampling test runs (class, model): %s" % missing
+
+
+# teeth: the draw checker of the GPU test applied on the CPU to a numpy model of the kernel — fp32 e (np.exp standing in
+# for __expf), top-k / top-p thresholds over 2^-40 fixed-point masses, and FP32Draw's orders — right, or wrong in one way.
+def _model_sample(logits, T, k, p, step, fallback="span", carry=True, strict_k=False, p_short=False, p_zero_off=False,
+                  step_shift=0):
+    if not T > 0:
+        return int(np.argmax(logits))
+    e = SS.kernel_e(logits, T)
+    keep = np.ones(e.size, bool)
+    if 0 < k < e.size:
+        kth = np.sort(e)[::-1][k - 1]
+        keep = e > kth if strict_k else e >= kth
+    if p < 1.0 and not (p_zero_off and p <= 0):
+        q = np.floor(np.where(keep, e, 0).astype(np.float64) * 2.0 ** 40)
+        vals = np.unique(e[keep])[::-1]                                      # descending
+        cum = np.cumsum([q[keep & (e == v)].sum() for v in vals]) if vals.size < 64 else \
+            np.cumsum(np.bincount(np.searchsorted(-vals, -e[keep]), weights=q[keep], minlength=vals.size))
+        i = int(np.searchsorted(cum, np.floor(p * cum[-1]), side="left"))
+        i = min(i, vals.size - 1)
+        if p_short and i > 0:
+            i -= 1
+        keep &= e >= vals[i]
+    ek = np.where(keep, e, np.float32(0))
+    d = SS.FP32Draw(ek, carry=carry)
+    last_kept = int(np.nonzero(keep)[0][-1])
+    fb = (lambda w: d.last_positive(w) if w is not None else 0) if fallback == "span" else (lambda w: last_kept)
+    return d.draw(SS.u_of(step + step_shift), fb)
+
+
+def _model_rejects(cases, **knobs):
+    """Draws of the model the checker rejects, over cases [(logits, T, k, p, steps)]."""
+    bad = 0
+    for row, T, k, p, steps in cases:
+        ref = SS.Ref(row, T, k, p)
+        for s in steps:
+            bad += not ref.check(_model_sample(row, T, k, p, int(s), **knobs), SS.u_of(s))[0]
+    return bad
+
+
+def _teeth_cases():
+    rs = np.random.RandomState(12)
+    out = []
+    for V in (SS.VOCAB_LLAMA3, SS.VOCAB_ODD):
+        lm, tied = SS.make_row("lm", V, 3), SS.make_row("tiedk", V, 4)
+        out += [(lm, 1.0, 0, 1.0, rs.randint(0, SS.N_STEPS, 24)), (lm, 0.7, 0, 0.0, rs.randint(0, SS.N_STEPS, 8)),
+                (tied, 1.0, SS.TIED_K, 1.0, rs.randint(0, SS.N_STEPS, 48)), (tied, 1.0, 0, 0.9, rs.randint(0, SS.N_STEPS, 48))]
+    return out
+
+
+def _gap_cases():
+    out = []
+    for V, where in SS.GAP_CASES:
+        row = SS.crafted_gap_row(V, 16 if where == "mid" else (V - 1) // SS.span_of(V))
+        out.append((row, 1.0, 0, 1.0, SS.gap_steps(SS.kernel_e(row, 1.0), per_warp=16)))
+    return out
+
+
+def test_sampler_checker_accepts_a_correct_kernel_model():
+    cases = _teeth_cases() + _gap_cases()
+    for V in (SS.VOCAB_TINY, SS.VOCAB_ODD):
+        rs = np.random.RandomState(V)
+        for kind, seed, T, k, p in SS.case_list(V)[::3]:
+            row = SS.make_row(kind, V, seed)
+            cases.append((row, T, k, p, np.concatenate([SS.Ref(row, T, k, p).directed_steps(rs, 2), rs.randint(0, SS.N_STEPS, 2)])))
+    assert _model_rejects(cases) == 0
+
+
+def test_sampler_checker_rejects_the_fallback_to_the_last_kept_index_on_gap_draws():
+    """The kernel's old fallback: a target in the gap between the crossing warp's total and its row scans crossed no lane,
+    and the draw became the last index with key >= floor_key — vocab - 1 whenever no top-k / top-p was set."""
+    cases = _gap_cases()
+    assert all(len(c[4]) >= 4 for c in cases)
+    for row, T, k, p, steps in cases:
+        assert all(_model_sample(row, T, k, p, int(s), fallback="last_kept") == row.size - 1 for s in steps)
+        assert _model_rejects([(row, T, k, p, steps)], fallback="last_kept") == len(steps)
+
+
+def test_sampler_checker_rejects_a_dropped_run_carry_a_strict_top_k_a_short_top_p_a_shifted_counter_and_top_p_0_off():
+    cases = _teeth_cases()
+    lm_t1 = [c for c in cases if c[1] == 1.0 and c[2] == 0 and c[3] == 1.0]
+    assert _model_rejects(lm_t1, carry=False) > 0
+    assert _model_rejects([c for c in cases if c[2] == SS.TIED_K], strict_k=True) > 0
+    assert _model_rejects([c for c in cases if c[3] == 0.9], p_short=True) > 0
+    assert _model_rejects(lm_t1, step_shift=1) > 0
+    assert _model_rejects([c for c in cases if c[3] == 0.0], p_zero_off=True) > 0
