@@ -10,6 +10,7 @@ use std::time::Duration;
 
 pub const LLMLB_ABI_VERSION: u32 = 1;
 pub const LLMLB_IPC_HANDLE_BYTES: usize = 64;
+pub const LLMLB_MAX_TOP_LOGPROBS: usize = 20;
 
 pub const LLMLB_OK: c_int = 0;
 pub const LLMLB_E_INVALID_ARG: c_int = -1;
@@ -140,6 +141,16 @@ pub struct llmlb_token_event {
     pub t_ms: f64,
 }
 
+/// Logprobs of one token event (`llmlb_request_poll_logprobs`): log_softmax of the row the sampler read.
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct llmlb_token_logprobs {
+    pub logprob: f32,
+    pub n_top: u32,
+    pub top_ids: [i32; 20],
+    pub top_logprobs: [f32; 20],
+}
+
 extern "C" {
     pub fn llmlb_abi_version() -> u32;
     pub fn llmlb_last_error() -> *const c_char;
@@ -155,7 +166,9 @@ extern "C" {
     pub fn llmlb_engine_pause(e: *mut llmlb_engine, paused: u32) -> c_int;
     pub fn llmlb_request_submit(e: *mut llmlb_engine, prompt_ids: *const i32, n_prompt: u32, s: *const llmlb_sampling, req_id: *mut u64) -> c_int;
     pub fn llmlb_request_submit_penalized(e: *mut llmlb_engine, prompt_ids: *const i32, n_prompt: u32, s: *const llmlb_sampling, pen: *const llmlb_penalties, req_id: *mut u64) -> c_int;
+    pub fn llmlb_request_submit_logprobs(e: *mut llmlb_engine, prompt_ids: *const i32, n_prompt: u32, s: *const llmlb_sampling, pen: *const llmlb_penalties, top_logprobs: u32, req_id: *mut u64) -> c_int;
     pub fn llmlb_request_poll(e: *mut llmlb_engine, req_id: u64, out: *mut llmlb_token_event, cap: u32, n_out: *mut u32, timeout_ms: c_int) -> c_int;
+    pub fn llmlb_request_poll_logprobs(e: *mut llmlb_engine, req_id: u64, out: *mut llmlb_token_event, lp: *mut llmlb_token_logprobs, cap: u32, n_out: *mut u32, timeout_ms: c_int) -> c_int;
     pub fn llmlb_request_cancel(e: *mut llmlb_engine, req_id: u64) -> c_int;
     pub fn llmlb_request_release(e: *mut llmlb_engine, req_id: u64) -> c_int;
 }

@@ -202,6 +202,29 @@ typedef struct llmlb_penalties {
  * penalised: it runs exactly as through llmlb_request_submit. */
 int llmlb_request_submit_penalized(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt,
                                    const llmlb_sampling* s, const llmlb_penalties* pen, uint64_t* req_id);
+
+/* OpenAI's logprobs / top_logprobs.  After each sampled token the engine reports log_softmax(z) over the whole
+ * vocabulary, where z is exactly the row the sampler reads: after the penalties and logit bias above (a +100 bias
+ * gives that token a logprob of about 0), before temperature, top-k and top-p (logprobs do not depend on them).
+ * In fp32 on the row:  m = max z,  s = sum_j expf(z_j - m) (accurate expf; the terms are summed in fp64 and rounded
+ * once to fp32),  logprob_j = (z_j - m) - logf(s)  (not z_j - lse: large logits do not cancel; -inf stays -inf).
+ * The top list holds the n = min(top_logprobs, vocab) largest z, by descending z with ties by ascending token id.
+ * The event token's logprob comes from the same expression, so it equals its list entry bit for bit. */
+#define LLMLB_MAX_TOP_LOGPROBS 20
+typedef struct llmlb_token_logprobs {
+  float logprob;                              /* of the event's token_id */
+  uint32_t n_top;                             /* min(top_logprobs, vocab); 0 on an event with token_id < 0 */
+  int32_t top_ids[LLMLB_MAX_TOP_LOGPROBS];    /* descending z, ties by ascending id */
+  float top_logprobs[LLMLB_MAX_TOP_LOGPROBS];
+} llmlb_token_logprobs;
+/* llmlb_request_submit_penalized (pen NULL = none) for a request that reports logprobs with top_logprobs (0..20)
+ * alternatives per token; top_logprobs > 20 returns LLMLB_E_INVALID_ARG. */
+int llmlb_request_submit_logprobs(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt, const llmlb_sampling* s,
+                                  const llmlb_penalties* pen, uint32_t top_logprobs, uint64_t* req_id);
+/* llmlb_request_poll that also returns lp[i] for out[i] (same queue: either call drains it).  For a request
+ * submitted without logprobs, and for an event with token_id < 0, lp[i] has logprob = NaN and n_top = 0. */
+int llmlb_request_poll_logprobs(llmlb_engine* e, uint64_t req_id, llmlb_token_event* out, llmlb_token_logprobs* lp,
+                                uint32_t cap, uint32_t* n_out, int timeout_ms);
 /* Drain up to cap events. timeout_ms: 0 = return at once, <0 = wait until at least one. */
 int llmlb_request_poll(llmlb_engine* e, uint64_t req_id, llmlb_token_event* out, uint32_t cap,
                        uint32_t* n_out, int timeout_ms);
@@ -316,6 +339,11 @@ int llmlb_op_sample(const float* logits, uint32_t n_rows, uint32_t vocab, const 
 int llmlb_op_penalize(float* logits, uint32_t n_rows, uint32_t vocab, const int32_t* counts, uint64_t count_stride,
                       const float* freq, const float* pres, const int32_t* bias_ids, const float* bias_vals,
                       const uint32_t* n_bias, uint32_t bias_stride, void* stream);
+/* Logprobs of R rows (the kernel the engine launches after sampling; definition at llmlb_token_logprobs).  Row r
+ * reports tokens[r] and min(top_n[r], vocab, 20) alternatives into out_records[r]; top_n[r] < 0 skips the row and
+ * leaves its record untouched. */
+int llmlb_op_logprobs(const float* logits, uint32_t n_rows, uint32_t vocab, const int32_t* tokens,
+                      const int32_t* top_n, llmlb_token_logprobs* out_records, void* stream);
 /* a2.13 all-reduce(sum) of fp32 [n] across tp ranks through peer-mapped buffers. */
 int llmlb_op_allreduce(llmlb_engine* e, float* buf_f32, uint64_t n, void* stream);
 

@@ -6,8 +6,9 @@
 // token-event queues for non-blocking submit/poll/cancel.  Device side: the kernels in the
 // sibling .cu files, chained on one stream; decode steps are captured into CUDA graphs per batch
 // width and all per-sequence decode state (length, last token, sampler counters, the token counts
-// and bias list of frequency / presence penalties) lives in HBM so the GPU never waits for the
-// host between tokens — the host reads tokens `lookahead` steps late.
+// and bias list of frequency / presence penalties, the number of logprob alternatives) lives in HBM
+// so the GPU never waits for the host between tokens — the host reads tokens (and the logprob
+// records of the requests that asked for them) `lookahead` steps late.
 #include <cuda.h>
 
 #include <algorithm>
@@ -17,6 +18,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <deque>
+#include <limits>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -81,6 +83,8 @@ int penalty_count_launch(int32_t* counts, uint64_t count_stride, const float* fr
                          const int32_t* row_slot, const int32_t* out_ids, uint32_t n_rows, cudaStream_t st);
 int penalty_reset_launch(int32_t* counts, uint64_t count_stride, float* freq, float* pres, uint32_t* n_bias, int32_t slot,
                          float f, float p, uint32_t nb, uint32_t vocab, const int32_t* gen, uint32_t n_gen, cudaStream_t st);
+int logprob_launch(const float* logits, uint32_t n_rows, uint32_t vocab, const int32_t* tokens, const int32_t* top_n,
+                   const int32_t* row_slot, llmlb_token_logprobs* out, cudaStream_t st);
 int rope_append_launch(void* qkv, const int32_t* positions, const int32_t* page_of_token, const float* rope_table,
                        void* k_pages, void* v_pages, uint32_t n_tokens, uint32_t n_heads, uint32_t n_kv, bool pdl,
                        cudaStream_t st);
@@ -125,6 +129,7 @@ struct SlotState {  // per-sequence decode state, device resident
   float* pen_freq;      // penalties (penalty.cu): both 0 and no bias = the slot is not penalised
   float* pen_pres;
   uint32_t* pen_n_bias;
+  int32_t* lp_top;      // logprobs (logprob.cu): alternatives per token, -1 = the slot reports no logprobs
 };
 struct BatchView {  // compact per-step arrays
   int32_t* slots;     // batch position -> slot
@@ -189,6 +194,7 @@ struct Request {
   float freq_pen = 0.f, pres_pen = 0.f;
   std::vector<int32_t> bias_ids;
   std::vector<float> bias_vals;
+  int32_t top_logprobs = -1;   // logprobs with this many alternatives (0..20), -1 = none (logprob.cu)
   int slot = -1;
   std::vector<int32_t> pages;
   uint32_t prefilled = 0;   // context tokens whose KV is (being) written
@@ -208,6 +214,7 @@ struct Request {
   bool client_released = false;
   uint32_t finish_reason = LLMLB_FINISH_NONE;
   std::deque<llmlb_token_event> events;
+  std::deque<llmlb_token_logprobs> lp_events;   // logprob requests: one per entry of `events`
   std::chrono::steady_clock::time_point t_submit;
 };
 using ReqPtr = std::shared_ptr<Request>;
@@ -215,6 +222,7 @@ using ReqPtr = std::shared_ptr<Request>;
 struct InflightStep {
   cudaEvent_t ev_start = nullptr, ev_end = nullptr;
   int32_t* host_ids = nullptr;        // pinned
+  const llmlb_token_logprobs* host_lp = nullptr;   // pinned; set when some row of the step reports logprobs
   std::vector<ReqPtr> reqs;           // batch position -> request
   bool is_prefill = false;
   uint32_t n_tokens = 0;
@@ -394,11 +402,13 @@ struct llmlb_engine {
   int32_t* pen_bias_ids = nullptr;
   float* pen_bias_vals = nullptr;
   int32_t* pen_gen = nullptr;
+  llmlb_token_logprobs* d_lp = nullptr;   // logprob records of the step's rows [max_seqs]
   static constexpr int kRing = 8;
   uint8_t* h_stage[kRing] = {};
   size_t stage_bytes = 0;
   uint64_t stage_seq = 0;
   int32_t* h_out[kRing] = {};
+  llmlb_token_logprobs* h_lp[kRing] = {};   // beside h_out[i]: the records of logprob steps
   uint64_t out_seq = 0;
   std::vector<cudaEvent_t> ev_pool;
 
@@ -417,7 +427,8 @@ struct llmlb_engine {
   __nv_bfloat16* ylast = nullptr;    // [max_seqs][hidden] normalised rows that need logits (protocol B)
   CUtensorMap m_ylast[5]{};
 
-  // decode graphs by batch width, with bit 31 set when some sequence of the batch is penalised
+  // decode graphs by batch width, with bit 31 set when some sequence of the batch is penalised and bit 30 when some
+  // sequence reports logprobs
   std::unordered_map<uint32_t, cudaGraphExec_t> graphs;
   std::unordered_map<uint32_t, uint64_t> graph_nodes;  // kernels per captured step
   bool paused = false;
@@ -468,8 +479,9 @@ struct llmlb_engine {
   };
   int proj(const CUtensorMap& mw, const void* w, const void* xin, const CUtensorMap* mx, void* out, uint32_t T,
            uint32_t n_out, uint32_t k, uint32_t epi, uint32_t out_stride, int wait_coll = -1);
-  int layer_stack_decode(uint32_t nb, bool pen = false);
-  int launch_decode_step(uint32_t nb, bool pen);
+  int layer_stack_decode(uint32_t nb, bool pen = false, bool lp = false);
+  int launch_decode_step(uint32_t nb, bool pen, bool lp);
+  int logprob_rows(uint32_t R);          // after sampling: records of the rows whose slot reports logprobs
   int penalize_rows(uint32_t R);         // before sampling R rows of B (slots in B.slots)
   int count_sampled(uint32_t R);         // after sampling: each penalised row's token counts
   int forward_tokens(uint32_t T, bool decode, uint32_t nb, uint32_t n_tiles, FwdState* fs);
@@ -714,6 +726,7 @@ int llmlb_engine::alloc_all() {
   RC(dmalloc(&pen_counts, ms * M.vocab));   // int32: a count can pass 65535 at 128K context
   RC(dmalloc(&pen_bias_ids, ms * LLMLB_MAX_LOGIT_BIAS)); RC(dmalloc(&pen_bias_vals, ms * LLMLB_MAX_LOGIT_BIAS));
   RC(dmalloc(&pen_gen, cfg.max_ctx));
+  RC(dmalloc(&S.lp_top, ms)); RC(dmalloc(&d_lp, ms));
   RC(dmalloc(&B.slots, ms)); RC(dmalloc(&B.ids, ms)); RC(dmalloc(&B.seq_lens, ms));
   RC(dmalloc(&B.temperature, ms)); RC(dmalloc(&B.top_p, ms)); RC(dmalloc(&B.top_k, ms));
   RC(dmalloc(&B.seed, ms)); RC(dmalloc(&B.step, ms)); RC(dmalloc(&B.out_ids, ms));
@@ -722,6 +735,7 @@ int llmlb_engine::alloc_all() {
   for (int i = 0; i < kRing; ++i) {
     LLMLB_CUDA_CHECK(cudaHostAlloc((void**)&h_stage[i], stage_bytes, cudaHostAllocDefault));
     LLMLB_CUDA_CHECK(cudaHostAlloc((void**)&h_out[i], ms * 4, cudaHostAllocDefault));
+    LLMLB_CUDA_CHECK(cudaHostAlloc((void**)&h_lp[i], ms * sizeof(llmlb_token_logprobs), cudaHostAllocDefault));
   }
   if (tp == 1) RC(dmalloc(&part_ws, size_t(8) * t_cap * H, false));
   return LLMLB_OK;
@@ -1018,9 +1032,13 @@ int llmlb_engine::penalize_rows(uint32_t R) {
 int llmlb_engine::count_sampled(uint32_t R) {
   return penalty_count_launch(pen_counts, M.vocab, S.pen_freq, S.pen_pres, S.pen_n_bias, B.slots, B.out_ids, R, st);
 }
+int llmlb_engine::logprob_rows(uint32_t R) {
+  return logprob_launch(logits, R, M.vocab, B.out_ids, S.lp_top, B.slots, d_lp, st);
+}
 
-// pen: some sequence of the batch is penalised (the unpenalised step launches exactly what it did without penalties)
-int llmlb_engine::layer_stack_decode(uint32_t nb, bool pen) {
+// pen: some sequence of the batch is penalised, lp: some sequence reports logprobs (a step with neither launches
+// exactly what it did without penalties and logprobs)
+int llmlb_engine::layer_stack_decode(uint32_t nb, bool pen, bool lp) {
   decode_prepare_kernel<<<ceil_div(nb, 128), 128, 0, st>>>(S, B, nb);
   LLMLB_LAUNCH_CHECK();
   RC(llmlb_op_embed(embed, B.ids, x, nb, M.hidden, M.vocab, st));
@@ -1029,22 +1047,23 @@ int llmlb_engine::layer_stack_decode(uint32_t nb, bool pen) {
   RC(logits_after_forward(&fs, nb, true));
   if (pen) RC(penalize_rows(nb));
   RC(llmlb_op_sample(logits, nb, M.vocab, B.temperature, B.top_p, B.top_k, B.seed, B.step, B.out_ids, st));
+  if (lp) RC(logprob_rows(nb));
   step_finish_kernel<<<ceil_div(nb, 128), 128, 0, st>>>(S, B, nb);
   LLMLB_LAUNCH_CHECK();
   if (pen) RC(count_sampled(nb));
   return LLMLB_OK;
 }
 
-int llmlb_engine::launch_decode_step(uint32_t nb, bool pen) {
-  if (!cfg.use_cuda_graphs) return layer_stack_decode(nb, pen);
-  const uint32_t key = nb | (pen ? 0x80000000u : 0u);
+int llmlb_engine::launch_decode_step(uint32_t nb, bool pen, bool lp) {
+  if (!cfg.use_cuda_graphs) return layer_stack_decode(nb, pen, lp);
+  const uint32_t key = nb | (pen ? 0x80000000u : 0u) | (lp ? 0x40000000u : 0u);
   auto it = graphs.find(key);
   if (it == graphs.end()) {
     // kernel attributes (max dynamic smem) were set by the eager warm-up in init()
     cudaGraph_t g = nullptr;
     uint64_t launches_before = g_kernel_launches.load();
     LLMLB_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    int rc = layer_stack_decode(nb, pen);
+    int rc = layer_stack_decode(nb, pen, lp);
     cudaError_t ce = cudaStreamEndCapture(st, &g);
     if (rc != LLMLB_OK) { if (g) cudaGraphDestroy(g); return rc; }
     if (ce != cudaSuccess) { set_error(std::string("graph capture: ") + cudaGetErrorString(ce)); return LLMLB_E_DEVICE; }
@@ -1067,7 +1086,7 @@ __global__ void iota_kernel(int32_t* p, uint32_t n) {
   if (i < n) p[i] = int32_t(i);
 }
 __global__ void slot_init_kernel(SlotState S, int32_t slot, float temperature, float top_p,
-                                 int32_t top_k, uint64_t seed, uint64_t step0) {
+                                 int32_t top_k, uint64_t seed, uint64_t step0, int32_t lp_top) {
   S.seq_len[slot] = 0;
   S.last_token[slot] = 0;
   S.temperature[slot] = temperature;
@@ -1078,6 +1097,7 @@ __global__ void slot_init_kernel(SlotState S, int32_t slot, float temperature, f
   S.pen_freq[slot] = 0.f;  // unpenalised; penalty_reset_kernel follows for a penalised request
   S.pen_pres[slot] = 0.f;
   S.pen_n_bias[slot] = 0;
+  S.lp_top[slot] = lp_top;  // -1 unless the request reports logprobs
 }
 __global__ void prefill_finish_kernel(SlotState S, BatchView B, uint32_t n) {
   uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1116,12 +1136,14 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
   step.n_tokens = T;
   uint32_t row = 0, n_tiles = 0, R = 0;
   bool pen_rows = false;   // some finished row is penalised
+  bool lp_rows = false;    // some finished row reports logprobs
   for (size_t i = 0; i < reqs.size(); ++i) {
     Request& r = *reqs[i];
     if (r.prefilled == 0) {  // first chunk: publish block table + sampler state
       LLMLB_CUDA_CHECK(cudaMemcpyAsync(d_block_tables + size_t(r.slot) * pages_per_seq, r.pages.data(),
                                        r.pages.size() * 4, cudaMemcpyHostToDevice, st));
-      slot_init_kernel<<<1, 1, 0, st>>>(S, r.slot, r.s.temperature, r.s.top_p, (int32_t)r.s.top_k, r.s.seed, uint64_t(r.harvested));
+      slot_init_kernel<<<1, 1, 0, st>>>(S, r.slot, r.s.temperature, r.s.top_p, (int32_t)r.s.top_k, r.s.seed, uint64_t(r.harvested),
+                                   r.top_logprobs);
       LLMLB_LAUNCH_CHECK();
       if (r.penalized) {   // bias list into the slot's rows; counts = the tokens generated before a preemption (none otherwise)
         const uint32_t nb = uint32_t(r.bias_ids.size());
@@ -1154,6 +1176,7 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
       s_slots[R] = r.slot;
       s_lens[R] = int32_t(r.prompt.size());
       pen_rows |= r.penalized;
+      lp_rows |= r.top_logprobs >= 0;
       step.reqs.push_back(reqs[i]);
       ++R;
     }
@@ -1189,13 +1212,19 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
     LLMLB_LAUNCH_CHECK();
     if (pen_rows) RC(penalize_rows(R));
     RC(llmlb_op_sample(logits, R, M.vocab, B.temperature, B.top_p, B.top_k, B.seed, B.step, B.out_ids, st));
+    if (lp_rows) RC(logprob_rows(R));
     step_finish_kernel<<<ceil_div(R, 128), 128, 0, st>>>(S, B, R);
     LLMLB_LAUNCH_CHECK();
     if (pen_rows) RC(count_sampled(R));
     prefill_finish_kernel<<<ceil_div(R, 128), 128, 0, st>>>(S, B, R);
     LLMLB_LAUNCH_CHECK();
-    step.host_ids = h_out[(out_seq++) % kRing];
+    const uint64_t ring = (out_seq++) % kRing;
+    step.host_ids = h_out[ring];
     LLMLB_CUDA_CHECK(cudaMemcpyAsync(step.host_ids, B.out_ids, R * 4, cudaMemcpyDeviceToHost, st));
+    if (lp_rows) {
+      step.host_lp = h_lp[ring];
+      LLMLB_CUDA_CHECK(cudaMemcpyAsync(h_lp[ring], d_lp, R * sizeof(llmlb_token_logprobs), cudaMemcpyDeviceToHost, st));
+    }
   }
   LLMLB_CUDA_CHECK(cudaEventRecord(step.ev_end, st));
   {
@@ -1246,11 +1275,16 @@ int llmlb_engine::run_decode(const std::vector<ReqPtr>& batch) {
   step.ev_start = get_event();
   step.ev_end = get_event();
   LLMLB_CUDA_CHECK(cudaEventRecord(step.ev_start, st));
-  bool pen = false;
-  for (auto& r : batch) pen |= r->penalized;
-  RC(launch_decode_step(nb, pen));
-  step.host_ids = h_out[(out_seq++) % kRing];
+  bool pen = false, lp = false;
+  for (auto& r : batch) { pen |= r->penalized; lp |= r->top_logprobs >= 0; }
+  RC(launch_decode_step(nb, pen, lp));
+  const uint64_t ring = (out_seq++) % kRing;
+  step.host_ids = h_out[ring];
   LLMLB_CUDA_CHECK(cudaMemcpyAsync(step.host_ids, B.out_ids, nb * 4, cudaMemcpyDeviceToHost, st));
+  if (lp) {
+    step.host_lp = h_lp[ring];
+    LLMLB_CUDA_CHECK(cudaMemcpyAsync(h_lp[ring], d_lp, nb * sizeof(llmlb_token_logprobs), cudaMemcpyDeviceToHost, st));
+  }
   LLMLB_CUDA_CHECK(cudaEventRecord(step.ev_end, st));
   {
     std::lock_guard<std::mutex> lk(mu);
@@ -1287,6 +1321,13 @@ void llmlb_engine::preempt(ReqPtr r) {
   preemptions++;
 }
 
+// the record of an event that has no logprobs: a request without them, or an end event without a token
+static llmlb_token_logprobs no_logprobs() {
+  llmlb_token_logprobs lp{};
+  lp.logprob = std::numeric_limits<float>::quiet_NaN();
+  return lp;
+}
+
 void llmlb_engine::finish_request(ReqPtr r, uint32_t reason) {  // mu held
   if (r->finished) return;
   r->finished = true;
@@ -1303,6 +1344,7 @@ void llmlb_engine::finish_request(ReqPtr r, uint32_t reason) {  // mu held
       ev.completion_tokens = r->harvested;
       ev.t_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - r->t_submit).count();
       r->events.push_back(ev);
+      if (r->top_logprobs >= 0) r->lp_events.push_back(no_logprobs());
     }
   }
   release_resources(r);
@@ -1338,6 +1380,7 @@ void llmlb_engine::harvest_one() {
     ev.completion_tokens = r->harvested;
     ev.t_ms = std::chrono::duration<double, std::milli>(now - r->t_submit).count();
     r->events.push_back(ev);
+    if (r->top_logprobs >= 0) r->lp_events.push_back(step.host_lp ? step.host_lp[b] : no_logprobs());
     bool stop_hit = false;
     if (!r->s.ignore_eos)
       for (int32_t sid : r->stop_ids) stop_hit |= (sid == tok);
@@ -1525,7 +1568,9 @@ void llmlb_engine::loop_follower() {
           r->bias_ids.assign(reinterpret_cast<const int32_t*>(p), reinterpret_cast<const int32_t*>(p) + n_bias);
           r->bias_vals.assign(reinterpret_cast<const float*>(p + size_t(n_bias) * 4), reinterpret_cast<const float*>(p + size_t(n_bias) * 8));
           r->penalized = true;
+          p += size_t(n_bias) * 8;
         }
+        if (size_t(buf.data() + buf.size() - p) >= 4) memcpy(&r->top_logprobs, p, 4);   // a logprob request
         r->client_released = true;
         r->t_submit = std::chrono::steady_clock::now();
         std::lock_guard<std::mutex> lk(mu);
@@ -1616,11 +1661,13 @@ extern "C" void llmlb_engine_destroy(llmlb_engine* e) {
   F(e->d_ids); F(e->d_pos); F(e->d_page_of_tok); F(e->d_tiles); F(e->d_last_rows);
   F(e->S.seq_len); F(e->S.last_token); F(e->S.temperature); F(e->S.top_p); F(e->S.top_k); F(e->S.seed); F(e->S.step);
   F(e->S.pen_freq); F(e->S.pen_pres); F(e->S.pen_n_bias); F(e->pen_counts); F(e->pen_bias_ids); F(e->pen_bias_vals); F(e->pen_gen);
+  F(e->S.lp_top); F(e->d_lp);
   F(e->B.slots); F(e->B.ids); F(e->B.seq_lens); F(e->B.temperature); F(e->B.top_p); F(e->B.top_k);
   F(e->B.seed); F(e->B.step); F(e->B.out_ids);
   for (int i = 0; i < llmlb_engine::kRing; ++i) {
     if (e->h_stage[i]) cudaFreeHost(e->h_stage[i]);
     if (e->h_out[i]) cudaFreeHost(e->h_out[i]);
+    if (e->h_lp[i]) cudaFreeHost(e->h_lp[i]);
   }
   if (e->tp_ready)
     for (uint32_t r = 0; r < e->tp; ++r)
@@ -1694,6 +1741,9 @@ static int take_penalties(const llmlb_penalties* pen, uint32_t vocab, Request* r
   return LLMLB_OK;
 }
 
+static int submit_request(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt, const llmlb_sampling* s,
+                          const llmlb_penalties* pen, int32_t top_logprobs, uint64_t* req_id, const char* bad_arg);
+
 extern "C" int llmlb_request_submit(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt,
                                     const llmlb_sampling* s, uint64_t* req_id) {
   return llmlb_request_submit_penalized(e, prompt_ids, n_prompt, s, nullptr, req_id);
@@ -1701,8 +1751,26 @@ extern "C" int llmlb_request_submit(llmlb_engine* e, const int32_t* prompt_ids, 
 
 extern "C" int llmlb_request_submit_penalized(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt,
                                               const llmlb_sampling* s, const llmlb_penalties* pen, uint64_t* req_id) {
+  return submit_request(e, prompt_ids, n_prompt, s, pen, -1, req_id,
+                        pen ? "llmlb_request_submit_penalized: bad argument" : "llmlb_request_submit: bad argument");
+}
+
+extern "C" int llmlb_request_submit_logprobs(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt,
+                                             const llmlb_sampling* s, const llmlb_penalties* pen, uint32_t top_logprobs,
+                                             uint64_t* req_id) {
+  if (top_logprobs > LLMLB_MAX_TOP_LOGPROBS) {
+    set_error("llmlb_request_submit_logprobs: top_logprobs must be in [0, 20]");
+    return LLMLB_E_INVALID_ARG;
+  }
+  return submit_request(e, prompt_ids, n_prompt, s, pen, int32_t(top_logprobs), req_id,
+                        "llmlb_request_submit_logprobs: bad argument");
+}
+
+// top_logprobs: -1 = the request reports no logprobs
+static int submit_request(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt, const llmlb_sampling* s,
+                          const llmlb_penalties* pen, int32_t top_logprobs, uint64_t* req_id, const char* bad_arg) {
   if (!e || !prompt_ids || !s || !req_id || n_prompt == 0) {
-    set_error(pen ? "llmlb_request_submit_penalized: bad argument" : "llmlb_request_submit: bad argument");
+    set_error(bad_arg);
     return LLMLB_E_INVALID_ARG;
   }
   if (s->max_tokens == 0) { set_error("max_tokens must be > 0"); return LLMLB_E_INVALID_ARG; }
@@ -1717,6 +1785,7 @@ extern "C" int llmlb_request_submit_penalized(llmlb_engine* e, const int32_t* pr
   if (std::isnan(s->temperature) || std::isnan(s->top_p)) { set_error("temperature/top_p is NaN"); return LLMLB_E_INVALID_ARG; }
   auto r = std::make_shared<Request>();
   RC(take_penalties(pen, e->M.vocab, r.get()));
+  r->top_logprobs = top_logprobs;
   r->prompt.assign(prompt_ids, prompt_ids + n_prompt);
   r->n_prompt0 = n_prompt;
   r->s = *s;
@@ -1733,10 +1802,11 @@ extern "C" int llmlb_request_submit_penalized(llmlb_engine* e, const int32_t* pr
     e->requests[r->id] = r;
     e->waiting.push_back(r);
     *req_id = r->id;
-    if (e->plan_on) {   // id, sampling, prompt, stop ids and (penalised requests) the penalties travel to the followers in queue order
+    if (e->plan_on) {   // id, sampling, prompt, stop ids, (penalised requests) the penalties and (logprob requests)
+                        // top_logprobs travel to the followers in queue order
       const uint32_t n_bias = uint32_t(r->bias_ids.size());
       std::vector<uint8_t> rec(8 + sizeof(llmlb_sampling) + 8 + (size_t(n_prompt) + r->stop_ids.size()) * 4 +
-                               (r->penalized ? 12 + size_t(n_bias) * 8 : 0));
+                               (r->penalized ? 12 + size_t(n_bias) * 8 : 0) + (top_logprobs >= 0 ? 4 : 0));
       uint8_t* p = rec.data();
       memcpy(p, &r->id, 8); p += 8;
       memcpy(p, &r->s, sizeof(llmlb_sampling)); p += sizeof(llmlb_sampling);
@@ -1748,7 +1818,10 @@ extern "C" int llmlb_request_submit_penalized(llmlb_engine* e, const int32_t* pr
       if (r->penalized) {   // [f32 frequency][f32 presence][u32 n_bias][i32 ids][f32 values]
         memcpy(p, &r->freq_pen, 4); memcpy(p + 4, &r->pres_pen, 4); memcpy(p + 8, &n_bias, 4); p += 12;
         if (n_bias) { memcpy(p, r->bias_ids.data(), size_t(n_bias) * 4); memcpy(p + size_t(n_bias) * 4, r->bias_vals.data(), size_t(n_bias) * 4); }
+        p += size_t(n_bias) * 8;
       }
+      // [i32 top_logprobs]: 4 bytes, so a follower cannot take it for a penalty block (at least 12)
+      if (top_logprobs >= 0) memcpy(p, &top_logprobs, 4);
       e->plan_log(kPlanSubmit, rec.data(), uint32_t(rec.size()));
     }
   }
@@ -1759,6 +1832,12 @@ extern "C" int llmlb_request_submit_penalized(llmlb_engine* e, const int32_t* pr
 extern "C" int llmlb_request_poll(llmlb_engine* e, uint64_t req_id, llmlb_token_event* out,
                                   uint32_t cap, uint32_t* n_out, int timeout_ms) {
   if (!e || !out || !n_out || cap == 0) { set_error("llmlb_request_poll: bad argument"); return LLMLB_E_INVALID_ARG; }
+  return llmlb_request_poll_logprobs(e, req_id, out, nullptr, cap, n_out, timeout_ms);
+}
+
+extern "C" int llmlb_request_poll_logprobs(llmlb_engine* e, uint64_t req_id, llmlb_token_event* out, llmlb_token_logprobs* lp,
+                                           uint32_t cap, uint32_t* n_out, int timeout_ms) {
+  if (!e || !out || !n_out || cap == 0) { set_error("llmlb_request_poll_logprobs: bad argument"); return LLMLB_E_INVALID_ARG; }
   *n_out = 0;
   std::unique_lock<std::mutex> lk(e->mu);
   auto it = e->requests.find(req_id);
@@ -1770,6 +1849,9 @@ extern "C" int llmlb_request_poll(llmlb_engine* e, uint64_t req_id, llmlb_token_
     else if (!e->cv_events.wait_for(lk, std::chrono::milliseconds(timeout_ms), ready)) return LLMLB_E_TIMEOUT;
   }
   while (*n_out < cap && !r->events.empty()) {
+    llmlb_token_logprobs rec = no_logprobs();
+    if (!r->lp_events.empty()) { rec = r->lp_events.front(); r->lp_events.pop_front(); }
+    if (lp) lp[*n_out] = rec;
     out[(*n_out)++] = r->events.front();
     r->events.pop_front();
   }
@@ -2056,7 +2138,7 @@ extern "C" int llmlb_debug_prefill_logits(llmlb_engine* e, const int32_t* prompt
   LLMLB_CUDA_CHECK(cudaMemcpy(e->d_pos, pos.data(), n * 4, cudaMemcpyHostToDevice));
   LLMLB_CUDA_CHECK(cudaMemcpy(e->d_page_of_tok, page.data(), n * 4, cudaMemcpyHostToDevice));
   LLMLB_CUDA_CHECK(cudaMemcpy(e->d_tiles, tiles.data(), tiles.size() * 4, cudaMemcpyHostToDevice));
-  slot_init_kernel<<<1, 1, 0, st>>>(e->S, slot, 0.f, 1.f, 0, 0, 0);
+  slot_init_kernel<<<1, 1, 0, st>>>(e->S, slot, 0.f, 1.f, 0, 0, 0, -1);
   LLMLB_LAUNCH_CHECK();
   RC(llmlb_op_embed(e->embed, e->d_ids, e->x, n, e->M.hidden, e->M.vocab, st));
   llmlb_engine::FwdState fs;

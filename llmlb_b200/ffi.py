@@ -66,6 +66,14 @@ class TokenEvent(C.Structure):
                 ("t_ms", C.c_double)]
 
 
+MAX_TOP_LOGPROBS = 20
+
+
+class TokenLogprobs(C.Structure):
+    _fields_ = [("logprob", C.c_float), ("n_top", C.c_uint32), ("top_ids", C.c_int32 * MAX_TOP_LOGPROBS),
+                ("top_logprobs", C.c_float * MAX_TOP_LOGPROBS)]
+
+
 u32, u64, i32, f32, vp, cp = C.c_uint32, C.c_uint64, C.c_int32, C.c_float, C.c_void_p, C.c_char_p
 _P = C.POINTER
 
@@ -84,7 +92,9 @@ PROTOTYPES = {
     "llmlb_engine_pause": (C.c_int, [vp, u32]),
     "llmlb_request_submit": (C.c_int, [vp, _P(i32), u32, _P(Sampling), _P(u64)]),
     "llmlb_request_submit_penalized": (C.c_int, [vp, _P(i32), u32, _P(Sampling), _P(Penalties), _P(u64)]),
+    "llmlb_request_submit_logprobs": (C.c_int, [vp, _P(i32), u32, _P(Sampling), _P(Penalties), u32, _P(u64)]),
     "llmlb_request_poll": (C.c_int, [vp, u64, _P(TokenEvent), u32, _P(u32), C.c_int]),
+    "llmlb_request_poll_logprobs": (C.c_int, [vp, u64, _P(TokenEvent), _P(TokenLogprobs), u32, _P(u32), C.c_int]),
     "llmlb_request_cancel": (C.c_int, [vp, u64]),
     "llmlb_request_release": (C.c_int, [vp, u64]),
     "llmlb_debug_prefill_logits": (C.c_int, [vp, _P(i32), u32, _P(f32), _P(f32)]),
@@ -108,6 +118,7 @@ PROTOTYPES = {
                                             u32, u32, vp, vp]),
     "llmlb_op_sample": (C.c_int, [vp, u32, u32, vp, vp, vp, vp, vp, vp, vp]),
     "llmlb_op_penalize": (C.c_int, [vp, u32, u32, vp, u64, vp, vp, vp, vp, vp, u32, vp]),
+    "llmlb_op_logprobs": (C.c_int, [vp, u32, u32, vp, vp, vp, vp]),
     "llmlb_op_allreduce": (C.c_int, [vp, vp, u64, vp]),
     "llmlb_op_synth_bf16": (C.c_int, [vp, u64, u64, u64, u64, u64, u64, u32, f32, vp]),
 }
@@ -218,10 +229,12 @@ class Engine:
 
     # ---- requests ----
     def submit(self, prompt_ids, max_tokens, temperature=0.0, top_k=0, top_p=1.0, seed=0,
-               stop_ids=(), ignore_eos=False, frequency_penalty=None, presence_penalty=None, logit_bias=None):
+               stop_ids=(), ignore_eos=False, frequency_penalty=None, presence_penalty=None, logit_bias=None,
+               logprobs=None):
         """frequency_penalty / presence_penalty / logit_bias ({token id: value}): OpenAI's penalties, applied on the device
         before sampling (llmlb_penalties).  Given at all (even neutral), the request goes through
-        llmlb_request_submit_penalized."""
+        llmlb_request_submit_penalized.  logprobs (0..20 alternatives per token; None = off): the request reports
+        logprobs (llmlb_token_logprobs, read with poll_logprobs) and goes through llmlb_request_submit_logprobs."""
         n = len(prompt_ids)
         arr = (i32 * n)(*prompt_ids)
         s = Sampling()
@@ -232,7 +245,10 @@ class Engine:
         s.ignore_eos = 1 if ignore_eos else 0
         rid = u64()
         if frequency_penalty is None and presence_penalty is None and logit_bias is None:
-            check(lib().llmlb_request_submit(self._h, arr, n, C.byref(s), C.byref(rid)))
+            if logprobs is None:
+                check(lib().llmlb_request_submit(self._h, arr, n, C.byref(s), C.byref(rid)))
+            else:
+                check(lib().llmlb_request_submit_logprobs(self._h, arr, n, C.byref(s), None, int(logprobs), C.byref(rid)))
             return rid.value
         bias = list((logit_bias or {}).items())
         ids = (i32 * max(1, len(bias)))(*[int(k) for k, _ in bias])
@@ -241,7 +257,10 @@ class Engine:
         pen.frequency_penalty = frequency_penalty or 0.0
         pen.presence_penalty = presence_penalty or 0.0
         pen.bias_ids, pen.bias_values, pen.n_bias = C.cast(ids, _P(i32)), C.cast(vals, _P(f32)), len(bias)
-        check(lib().llmlb_request_submit_penalized(self._h, arr, n, C.byref(s), C.byref(pen), C.byref(rid)))
+        if logprobs is None:
+            check(lib().llmlb_request_submit_penalized(self._h, arr, n, C.byref(s), C.byref(pen), C.byref(rid)))
+        else:
+            check(lib().llmlb_request_submit_logprobs(self._h, arr, n, C.byref(s), C.byref(pen), int(logprobs), C.byref(rid)))
         return rid.value
 
     def poll(self, rid, cap=256, timeout_ms=0):
@@ -255,12 +274,27 @@ class Engine:
                      prompt_tokens=e.prompt_tokens, completion_tokens=e.completion_tokens,
                      t_ms=e.t_ms) for e in buf[:n.value]]
 
+    def poll_logprobs(self, rid, cap=256, timeout_ms=0):
+        """poll, with each event's logprob (NaN without one) and top_logprobs: [(token id, logprob)], best first."""
+        buf = (TokenEvent * cap)()
+        lp = (TokenLogprobs * cap)()
+        n = u32()
+        rc = lib().llmlb_request_poll_logprobs(self._h, rid, buf, lp, cap, C.byref(n), timeout_ms)
+        if rc == E_TIMEOUT:
+            return []
+        check(rc)
+        return [dict(token_id=e.token_id, index=e.index, finish_reason=e.finish_reason,
+                     prompt_tokens=e.prompt_tokens, completion_tokens=e.completion_tokens, t_ms=e.t_ms,
+                     logprob=r.logprob, top_logprobs=[(r.top_ids[i], r.top_logprobs[i]) for i in range(r.n_top)])
+                for e, r in zip(buf[:n.value], lp[:n.value])]
+
     def generate(self, prompt_ids, max_tokens, **kw):
-        """submit + drain; returns (token ids, events)."""
+        """submit + drain; returns (token ids, events).  With logprobs=, the events carry them (poll_logprobs)."""
         rid = self.submit(prompt_ids, max_tokens, **kw)
+        poll = self.poll if kw.get("logprobs") is None else self.poll_logprobs
         toks, evs = [], []
         while True:
-            got = self.poll(rid, timeout_ms=-1)
+            got = poll(rid, timeout_ms=-1)
             evs.extend(got)
             for e in got:
                 if e["token_id"] >= 0:

@@ -2,6 +2,7 @@
 #include "gateway.hpp"
 
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 
 namespace llmlb_host {
@@ -516,12 +517,13 @@ std::string sha256_hex(const std::string& data) {
 std::string sse_event(const Json& j) { return "data: " + j.dump() + "\n\n"; }
 
 Json chat_chunk(const std::string& id, const std::string& model, int64_t created,
-                const std::string* role, const std::string* content, const char* finish_reason) {
+                const std::string* role, const std::string* content, const char* finish_reason, const Json* logprobs) {
   Json delta = Json::object();
   if (role) delta.set("role", *role);
   if (content) delta.set("content", *content);
   Json choice = Json::object();
   choice.set("index", 0); choice.set("delta", delta);
+  if (logprobs) choice.set("logprobs", *logprobs);
   choice.set("finish_reason", finish_reason ? Json(finish_reason) : Json());
   Json root = Json::object();
   root.set("id", id); root.set("object", "chat.completion.chunk"); root.set("created", created);
@@ -542,10 +544,12 @@ Json chat_usage_chunk(const std::string& id, const std::string& model, int64_t c
   return root;
 }
 Json chat_completion_body(const std::string& id, const std::string& model, int64_t created,
-                          const std::string& content, const char* finish_reason, uint32_t p, uint32_t c) {
+                          const std::string& content, const char* finish_reason, uint32_t p, uint32_t c, const Json* logprobs) {
   Json msg = Json::object(); msg.set("role", "assistant"); msg.set("content", content);
   Json choice = Json::object();
-  choice.set("index", 0); choice.set("message", msg); choice.set("finish_reason", finish_reason ? Json(finish_reason) : Json());
+  choice.set("index", 0); choice.set("message", msg);
+  if (logprobs) choice.set("logprobs", *logprobs);
+  choice.set("finish_reason", finish_reason ? Json(finish_reason) : Json());
   Json choices = Json::array(); choices.push(choice);
   Json root = Json::object();
   root.set("id", id); root.set("object", "chat.completion"); root.set("created", created); root.set("model", model);
@@ -553,18 +557,21 @@ Json chat_completion_body(const std::string& id, const std::string& model, int64
   return root;
 }
 Json completion_body(const std::string& id, const std::string& model, int64_t created,
-                     const std::string& text, const char* finish_reason, uint32_t p, uint32_t c) {
+                     const std::string& text, const char* finish_reason, uint32_t p, uint32_t c, const Json* logprobs) {
   Json choice = Json::object();
-  choice.set("index", 0); choice.set("text", text); choice.set("finish_reason", finish_reason ? Json(finish_reason) : Json());
+  choice.set("index", 0); choice.set("text", text);
+  if (logprobs) choice.set("logprobs", *logprobs);
+  choice.set("finish_reason", finish_reason ? Json(finish_reason) : Json());
   Json choices = Json::array(); choices.push(choice);
   Json root = Json::object();
   root.set("id", id); root.set("object", "text_completion"); root.set("created", created); root.set("model", model);
   root.set("choices", choices); root.set("usage", chat_usage(p, c));
   return root;
 }
-Json completion_chunk(const std::string& id, const std::string& model, int64_t created, const std::string* text, const char* finish_reason) {
+Json completion_chunk(const std::string& id, const std::string& model, int64_t created, const std::string* text, const char* finish_reason,
+                      const Json* logprobs) {
   Json choice = Json::object();
-  choice.set("index", 0); choice.set("text", text ? *text : std::string()); choice.set("logprobs", Json());
+  choice.set("index", 0); choice.set("text", text ? *text : std::string()); choice.set("logprobs", logprobs ? *logprobs : Json());
   choice.set("finish_reason", finish_reason ? Json(finish_reason) : Json());
   Json choices = Json::array(); choices.push(choice);
   Json root = Json::object();
@@ -578,6 +585,46 @@ Json completion_usage_chunk(const std::string& id, const std::string& model, int
   root.set("model", model); root.set("choices", Json::array()); root.set("usage", chat_usage(p, c));
   return root;
 }
+// OpenAI writes a log-probability it cannot represent (-inf) as -9999.0
+static Json logprob_value(float v) { return Json(std::isfinite(v) ? double(v) : -9999.0); }
+static Json logprob_bytes(const std::string& b) {
+  Json a = Json::array();
+  for (unsigned char c : b) a.push(Json(int(c)));
+  return a;
+}
+static Json chat_logprob_token(const LogprobToken& t) {
+  Json j = Json::object();
+  j.set("token", t.token); j.set("logprob", logprob_value(t.logprob)); j.set("bytes", logprob_bytes(t.bytes));
+  return j;
+}
+Json chat_logprobs(const std::vector<LogprobEntry>& entries) {
+  Json content = Json::array();
+  for (const auto& e : entries) {
+    Json j = chat_logprob_token(e.tok);
+    Json top = Json::array();
+    for (const auto& t : e.top) top.push(chat_logprob_token(t));
+    j.set("top_logprobs", top);
+    content.push(j);
+  }
+  Json root = Json::object();
+  root.set("content", content); root.set("refusal", Json());
+  return root;
+}
+Json completion_logprobs(const std::vector<LogprobEntry>& entries) {
+  Json tokens = Json::array(), lps = Json::array(), tops = Json::array(), offs = Json::array();
+  for (const auto& e : entries) {
+    tokens.push(e.tok.token);
+    lps.push(logprob_value(e.tok.logprob));
+    Json top = Json::object();   // two alternatives with the same text: the more probable one is kept
+    for (const auto& t : e.top) if (!top.get(t.token)) top.set(t.token, logprob_value(t.logprob));
+    tops.push(top);
+    offs.push(Json(e.text_offset));
+  }
+  Json root = Json::object();
+  root.set("tokens", tokens); root.set("token_logprobs", lps); root.set("top_logprobs", tops); root.set("text_offset", offs);
+  return root;
+}
+
 static Json resp_usage(uint32_t i, uint32_t o) {
   Json u = Json::object();
   u.set("input_tokens", i); u.set("output_tokens", o); u.set("total_tokens", i + o);

@@ -256,19 +256,39 @@ class StopMatcher {
 // ---- wire format writers (shapes pinned by the reference's fixtures, SURVEY.md §8b) ----
 std::string sse_event(const Json& j);                       // "data: {...}\n\n"
 inline std::string sse_done() { return "data: [DONE]\n\n"; }
+// logprobs (optional): the choice's "logprobs" value (chat_logprobs / completion_logprobs); without it the shapes are the
+// ones above, byte for byte
 Json chat_chunk(const std::string& id, const std::string& model, int64_t created,
-                const std::string* role, const std::string* content, const char* finish_reason);
+                const std::string* role, const std::string* content, const char* finish_reason,
+                const Json* logprobs = nullptr);
 Json chat_usage_chunk(const std::string& id, const std::string& model, int64_t created,
                       uint32_t prompt_tokens, uint32_t completion_tokens);
 Json chat_completion_body(const std::string& id, const std::string& model, int64_t created,
                           const std::string& content, const char* finish_reason,
-                          uint32_t prompt_tokens, uint32_t completion_tokens);
+                          uint32_t prompt_tokens, uint32_t completion_tokens, const Json* logprobs = nullptr);
 // legacy /v1/completions stream: {"object":"text_completion","choices":[{"index":0,"text":...,"finish_reason":...}]}
-Json completion_chunk(const std::string& id, const std::string& model, int64_t created, const std::string* text, const char* finish_reason);
+Json completion_chunk(const std::string& id, const std::string& model, int64_t created, const std::string* text, const char* finish_reason,
+                      const Json* logprobs = nullptr);
 Json completion_usage_chunk(const std::string& id, const std::string& model, int64_t created, uint32_t prompt_tokens, uint32_t completion_tokens);
 Json completion_body(const std::string& id, const std::string& model, int64_t created,
                      const std::string& text, const char* finish_reason, uint32_t prompt_tokens,
-                     uint32_t completion_tokens);
+                     uint32_t completion_tokens, const Json* logprobs = nullptr);
+
+// ---- OpenAI logprobs ----
+// One listed token (or one of its alternatives): text through from_utf8_lossy, raw bytes, log-probability.
+struct LogprobToken {
+  std::string token, bytes;
+  float logprob = 0.f;
+};
+struct LogprobEntry {
+  LogprobToken tok;
+  std::vector<LogprobToken> top;   // most probable first
+  uint32_t text_offset = 0;        // code points of completion text released before the token was fed
+};
+// chat: {"content":[{"token","logprob","bytes","top_logprobs":[{"token","logprob","bytes"}]}],"refusal":null}
+Json chat_logprobs(const std::vector<LogprobEntry>& entries);
+// completions: {"tokens":[...],"token_logprobs":[...],"top_logprobs":[{token: logprob}],"text_offset":[...]}
+Json completion_logprobs(const std::vector<LogprobEntry>& entries);
 Json responses_body(const std::string& id, const std::string& model, int64_t created,
                     const std::string& text, uint32_t input_tokens, uint32_t output_tokens,
                     const char* status);

@@ -38,6 +38,8 @@
 // unscaled), such as the scripted engine the CPU tests link it against.
 #pragma weak llmlb_engine_set_rope_freq_factors
 #pragma weak llmlb_request_submit_penalized
+#pragma weak llmlb_request_submit_logprobs
+#pragma weak llmlb_request_poll_logprobs
 #include "anthropic.hpp"
 #include "checkpoint.hpp"
 #include "download.hpp"
@@ -362,6 +364,40 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
   pen.bias_ids = bias_ids.data();
   pen.bias_values = bias_vals.data();
   pen.n_bias = uint32_t(bias_ids.size());
+  // OpenAI's logprobs.  Chat: "logprobs" true / false / null and "top_logprobs" 0..20 / null (only with logprobs: true).
+  // Completions: "logprobs" 0..5 / null, the legacy limit, and not with echo (prompt logprobs are not served).
+  bool lp_on = false;
+  uint32_t lp_top = 0;
+  if (kind == 0 && !anthropic) {
+    const Json* lp = req.get("logprobs");
+    const Json* tl = req.get("top_logprobs");
+    if (lp && !lp->is_null() && lp->type() != Json::Bool) { send_err(400, "logprobs must be a boolean", "invalid_request_error"); return; }
+    lp_on = lp && lp->as_bool();
+    if (tl && !tl->is_null()) {
+      if (!tl->is_number() || tl->as_double() != double(tl->as_int()) || tl->as_int() < 0 || tl->as_int() > LLMLB_MAX_TOP_LOGPROBS) {
+        send_err(400, "top_logprobs must be an integer in [0, 20]", "invalid_request_error");
+        return;
+      }
+      if (!lp_on) { send_err(400, "top_logprobs requires logprobs to be true", "invalid_request_error"); return; }
+      lp_top = uint32_t(tl->as_int());
+    }
+  } else if (kind == 2) {
+    const Json* lp = req.get("logprobs");
+    if (lp && !lp->is_null()) {
+      if (!lp->is_number() || lp->as_double() != double(lp->as_int()) || lp->as_int() < 0 || lp->as_int() > 5) {
+        send_err(400, "logprobs must be an integer in [0, 5]", "invalid_request_error");
+        return;
+      }
+      const Json* echo = req.get("echo");
+      if (echo && echo->as_bool()) { send_err(400, "echo together with logprobs is not supported: prompt logprobs are not served", "invalid_request_error"); return; }
+      lp_on = true;
+      lp_top = uint32_t(lp->as_int());
+    }
+  }
+  if (lp_on && !(llmlb_request_submit_logprobs && llmlb_request_poll_logprobs)) {
+    send_err(400, "logprobs are not supported by the engine library this server runs on", "invalid_request_error");
+    return;
+  }
   const bool stream = req.get("stream") && req.get("stream")->as_bool();
   bool include_usage = kind == 1;
   if (const Json* so = req.get("stream_options")) if (const Json* iu = so->get("include_usage")) include_usage = iu->as_bool();
@@ -370,6 +406,7 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
   const auto t0 = std::chrono::steady_clock::now();
   uint64_t rid = 0;
   int rc = !s.max_tokens ? LLMLB_E_INVALID_ARG
+           : lp_on        ? llmlb_request_submit_logprobs(G.eng, ids.data(), uint32_t(ids.size()), &s, penalized ? &pen : nullptr, lp_top, &rid)
            : penalized    ? llmlb_request_submit_penalized(G.eng, ids.data(), uint32_t(ids.size()), &s, &pen, &rid)
                           : llmlb_request_submit(G.eng, ids.data(), uint32_t(ids.size()), &s, &rid);
   if (rc == LLMLB_E_QUEUE_FULL) {   // openai.rs:841-861: 429 rate_limit_exceeded + Retry-After = queue timeout
@@ -408,10 +445,23 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
   std::string text;
   BpeTokenizer::Stream detok;
   uint32_t prompt_tokens = uint32_t(ids.size()), completion_tokens = 0, finish = LLMLB_FINISH_NONE;
+  // logprobs: every generated token fed to the text path is listed, except the stop ids (their text is skipped)
+  std::vector<LogprobEntry> lp_all;    // the whole list (response body)
+  size_t lp_sent = 0;                  // entries of lp_all already streamed
+  uint32_t text_cps = 0;               // code points of `text`
+  auto lp_token = [&](int32_t id, float v) {
+    LogprobToken t;
+    t.bytes = G.tok ? G.tok->token_bytes(id) : byte_detokenize(id);
+    t.token = G.tok ? BpeTokenizer::lossy_text(t.bytes) : t.bytes;
+    t.logprob = v;
+    return t;
+  };
+  auto lp_json = [&](const std::vector<LogprobEntry>& e) { return kind == 0 ? chat_logprobs(e) : completion_logprobs(e); };
   while (finish == LLMLB_FINISH_NONE) {
     llmlb_token_event ev[64];
+    llmlb_token_logprobs lpr[64];
     uint32_t got = 0;
-    rc = llmlb_request_poll(G.eng, rid, ev, 64, &got, 100);
+    rc = lp_on ? llmlb_request_poll_logprobs(G.eng, rid, ev, lpr, 64, &got, 100) : llmlb_request_poll(G.eng, rid, ev, 64, &got, 100);
     if (rc != LLMLB_OK && rc != LLMLB_E_TIMEOUT) { finish = LLMLB_FINISH_ERROR; break; }
     // a client that went away stops the generation, streamed or not — the reference's handler future is dropped with the
     // connection and its upstream request with it; a buffered response would otherwise run to its last token for nobody
@@ -424,8 +474,23 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
                                             : byte_detokenize(ev[i].token_id);
         // a stop string may span tokens: text that could still become one is held back
         const std::string piece = stopper.feed(raw_piece);
+        if (lp_on && !(!s.ignore_eos && std::find(G.stop_ids.begin(), G.stop_ids.end(), ev[i].token_id) != G.stop_ids.end())) {
+          LogprobEntry e;
+          e.tok = lp_token(ev[i].token_id, lpr[i].logprob);
+          for (uint32_t j = 0; j < lpr[i].n_top && j < LLMLB_MAX_TOP_LOGPROBS; ++j) e.top.push_back(lp_token(lpr[i].top_ids[j], lpr[i].top_logprobs[j]));
+          e.text_offset = text_cps;
+          lp_all.push_back(std::move(e));
+        }
         text += piece;
-        if (stream && !piece.empty()) out += kind == 1 ? sse_event(responses_event_delta(piece))
+        for (unsigned char c : piece) text_cps += (c & 0xC0) != 0x80;
+        if (stream && lp_on && (!piece.empty() || lp_sent < lp_all.size())) {
+          // held-back text (a split character, a possible stop prefix) still sends its entries, with empty text
+          const std::vector<LogprobEntry> fresh(lp_all.begin() + lp_sent, lp_all.end());
+          lp_sent = lp_all.size();
+          const Json lj = lp_json(fresh);
+          out += kind == 2 ? sse_event(completion_chunk(id, jm->str(), created, &piece, nullptr, &lj))
+                           : sse_event(chat_chunk(id, jm->str(), created, nullptr, &piece, nullptr, &lj));
+        } else if (stream && !piece.empty()) out += kind == 1 ? sse_event(responses_event_delta(piece))
                                      : kind == 2 ? sse_event(completion_chunk(id, jm->str(), created, &piece, nullptr))
                                      : sse_event(chat_chunk(id, jm->str(), created, nullptr, &piece, nullptr));
       }
@@ -505,9 +570,11 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
     const Json chat = chat_completion_body(id, jm->str(), created, text, fr, prompt_tokens, completion_tokens);
     send_json(fd, 200, openai_to_anthropic_message_response(chat, jm->str(), prompt_tokens, completion_tokens, "msg_" + std::to_string(n)).dump());
   } else {
-    Json body = kind == 0 ? chat_completion_body(id, jm->str(), created, text, fr, prompt_tokens, completion_tokens)
+    const Json lj = lp_on ? lp_json(lp_all) : Json();
+    const Json* lpp = lp_on ? &lj : nullptr;
+    Json body = kind == 0 ? chat_completion_body(id, jm->str(), created, text, fr, prompt_tokens, completion_tokens, lpp)
               : kind == 1 ? responses_body(id, jm->str(), created, text, prompt_tokens, completion_tokens, "completed")
-                          : completion_body(id, jm->str(), created, text, fr, prompt_tokens, completion_tokens);
+                          : completion_body(id, jm->str(), created, text, fr, prompt_tokens, completion_tokens, lpp);
     send_json(fd, 200, body.dump());
   }
 }

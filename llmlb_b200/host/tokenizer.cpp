@@ -512,6 +512,12 @@ std::string BpeTokenizer::decode_next(Stream* s, int32_t id, bool skip_special) 
   return ready;
 }
 
+std::string BpeTokenizer::token_bytes(int32_t id) const {
+  return id >= 0 && size_t(id) < id_to_bytes_.size() ? id_to_bytes_[id] : std::string();
+}
+
+std::string BpeTokenizer::lossy_text(const std::string& bytes) { return utf8_lossy(bytes); }
+
 std::string BpeTokenizer::flush(Stream* s) {
   std::string out = s->pending.empty() ? std::string() : std::string("\xEF\xBF\xBD");
   s->pending.clear();

@@ -39,6 +39,12 @@ class BpeTokenizer {
   std::string decode_next(Stream* s, int32_t id, bool skip_special) const;
   static std::string flush(Stream* s);
 
+  // Raw byte-level bytes of one token (a special token: its content; "" for an id outside the vocabulary), and those
+  // bytes as text the way decode_next releases it (every ill-formed or cut UTF-8 subpart becomes one U+FFFD): the
+  // `bytes` and `token` of an OpenAI logprobs entry.
+  std::string token_bytes(int32_t id) const;
+  static std::string lossy_text(const std::string& bytes);
+
   // <|begin_of_text|><|start_header_id|>{role}<|end_header_id|>\n\n{content|trim}<|eot_id|>...
   // followed by the assistant header when add_generation_prompt.
   std::string apply_chat_template(const std::vector<ChatMessage>& messages, bool add_generation_prompt) const;
