@@ -479,11 +479,10 @@ struct llmlb_engine {
   };
   int proj(const CUtensorMap& mw, const void* w, const void* xin, const CUtensorMap* mx, void* out, uint32_t T,
            uint32_t n_out, uint32_t k, uint32_t epi, uint32_t out_stride, int wait_coll = -1);
+  int decode_logits(uint32_t nb);        // a decode step's forward pass, up to its logits
   int layer_stack_decode(uint32_t nb, bool pen = false, bool lp = false);
   int launch_decode_step(uint32_t nb, bool pen, bool lp);
-  int logprob_rows(uint32_t R);          // after sampling: records of the rows whose slot reports logprobs
-  int penalize_rows(uint32_t R);         // before sampling R rows of B (slots in B.slots)
-  int count_sampled(uint32_t R);         // after sampling: each penalised row's token counts
+  int sample_rows(uint32_t R, bool pen, bool lp);   // logits of R rows of B -> B.out_ids (+ logprob records, penalty counts)
   int forward_tokens(uint32_t T, bool decode, uint32_t nb, uint32_t n_tiles, FwdState* fs);
   int forward_small_tp(uint32_t T, bool decode, uint32_t nb, uint32_t n_tiles, FwdState* fs);
   int forward_big_tp(uint32_t T, bool decode, uint32_t nb, uint32_t n_tiles, FwdState* fs);
@@ -491,10 +490,17 @@ struct llmlb_engine {
   int finish_small_tp(FwdState* fs, uint32_t T);                     // fold a pending collective: xres complete
   int logits_from_x(const float* src, uint32_t R);                   // fp32 rows, final norm applied here
   int logits_from_y(const __nv_bfloat16* src, const CUtensorMap* maps, uint32_t R);   // rows already normalised
-  int logits_tp_consume(FwdState* fs, uint32_t R);                   // protocol A: lm_head consumes the pending collective
-  int logits_gather(uint32_t R);                                     // tp > 1: vocab slices -> full rows
-  int logits_after_forward(FwdState* fs, uint32_t R, bool decode);   // rows = x[0..R) (decode) or gathered last rows
+  int step_logits(FwdState* fs, uint32_t R, bool decode);            // rows 0..R (decode) or the rows in d_last_rows
   float* logits_dst() { return tp == 1 ? logits : reinterpret_cast<float*>(xchg + logits_slot_off); }
+  // prefill-attention tiles of `take` rows from `row` on, holding positions p0.. of the sequence in `slot`
+  uint32_t add_tiles(int32_t* tiles, uint32_t n_tiles, uint32_t row, uint32_t take, uint32_t p0, int32_t slot) const {
+    for (uint32_t j = 0; j < take; j += pf_tile, ++n_tiles) {
+      int32_t* t = tiles + size_t(n_tiles) * 4;
+      t[0] = int32_t(row + j); t[1] = int32_t(std::min(pf_tile, take - j)); t[2] = int32_t(p0 + j); t[3] = slot;
+    }
+    return n_tiles;
+  }
+  int copy_out(InflightStep* step, uint32_t R, bool lp);   // the step's sampled ids (+ logprob records) into the output ring
   int run_prefill(const std::vector<ReqPtr>& reqs, const std::vector<uint32_t>& take);
   int run_decode(const std::vector<ReqPtr>& batch);
   void harvest_one();
@@ -973,85 +979,79 @@ int llmlb_engine::forward_big_tp(uint32_t T, bool decode, uint32_t nb, uint32_t 
 }
 
 // ---- logits ----
-int llmlb_engine::logits_gather(uint32_t R) {
-  if (tp == 1) return LLMLB_OK;
-  return ar_allgather_cols(tpc, logits_slot_off, logits, R, vocab_l, st);
-}
-// logits[r, :] for R fp32 residual rows at src (final RMSNorm applied here)
+// lm_head of R fp32 residual rows at src (final RMSNorm applied here) into this rank's vocabulary slice
 int llmlb_engine::logits_from_x(const float* src, uint32_t R) {
   const uint32_t H = M.hidden;
   float* dst = logits_dst();
-  if (R <= 4) {
-    RC(llmlb_op_gemv(lm_head, src, final_norm, M.rms_eps, dst, R, vocab_l, H, LLMLB_EPI_STORE_F32, vocab_l, st));
-  } else {
-    RC(llmlb_op_rmsnorm(src, final_norm, y, R, H, M.rms_eps, st));
-    RC(gemm_tc_launch(m_lm_head, m_y[bn_index(tc_pick_bn(R))], dst, R, vocab_l, H, LLMLB_EPI_STORE_F32, vocab_l, st, &m_y[bn_index(128)]));
-  }
-  return logits_gather(R);
+  if (R <= 4) return llmlb_op_gemv(lm_head, src, final_norm, M.rms_eps, dst, R, vocab_l, H, LLMLB_EPI_STORE_F32, vocab_l, st);
+  RC(llmlb_op_rmsnorm(src, final_norm, y, R, H, M.rms_eps, st));
+  return gemm_tc_launch(m_lm_head, m_y[bn_index(tc_pick_bn(R))], dst, R, vocab_l, H, LLMLB_EPI_STORE_F32, vocab_l, st, &m_y[bn_index(128)]);
 }
 // rows already normalised (bf16): the lm_head projection alone
 int llmlb_engine::logits_from_y(const __nv_bfloat16* src, const CUtensorMap* maps, uint32_t R) {
   const uint32_t H = M.hidden;
   float* dst = logits_dst();
-  if (R <= 4) RC(llmlb_op_gemv(lm_head, src, nullptr, M.rms_eps, dst, R, vocab_l, H, LLMLB_EPI_STORE_F32, vocab_l, st));
-  else RC(gemm_tc_launch(m_lm_head, maps[bn_index(tc_pick_bn(R))], dst, R, vocab_l, H, LLMLB_EPI_STORE_F32, vocab_l, st, &maps[bn_index(128)]));
-  return logits_gather(R);
+  if (R <= 4) return llmlb_op_gemv(lm_head, src, nullptr, M.rms_eps, dst, R, vocab_l, H, LLMLB_EPI_STORE_F32, vocab_l, st);
+  return gemm_tc_launch(m_lm_head, maps[bn_index(tc_pick_bn(R))], dst, R, vocab_l, H, LLMLB_EPI_STORE_F32, vocab_l, st, &maps[bn_index(128)]);
 }
-// protocol A, decode: the lm_head GEMV's prologue consumes the last down projection's collective
-int llmlb_engine::logits_tp_consume(FwdState* fs, uint32_t R) {
-  int rc = gemv_tp_consume(tpc, fs->pending_coll, lm_head, fs->xres, fs->xother, final_norm, M.rms_eps, logits_dst(), R,
-                           vocab_l, M.hidden, LLMLB_EPI_STORE_F32, vocab_l, tp_ll, tp_gather, st);
-  if (rc == LLMLB_E_UNSUPPORTED) {
-    RC(finish_small_tp(fs, R));
-    return logits_from_x(fs->xres, R);
-  }
-  RC(rc);
-  std::swap(fs->xres, fs->xother);
-  fs->pending = false;
-  return logits_gather(R);
-}
-// decode: logits of rows 0..R of the step; prefill: logits of the rows listed in d_last_rows
-int llmlb_engine::logits_after_forward(FwdState* fs, uint32_t R, bool decode) {
-  if (fs->y_final) {
-    if (decode) return logits_from_y(y, m_y, R);
-    gather_rows_bf16_kernel<<<R, 128, 0, st>>>(y, d_last_rows, ylast, M.hidden);
+// logits[r, :] of the step's final hidden rows: rows 0..R of a decode step, else the R rows listed in d_last_rows (a
+// prefill has folded its last protocol-A collective already: finish_small_tp)
+int llmlb_engine::step_logits(FwdState* fs, uint32_t R, bool decode) {
+  if (fs->y_final) {   // tp, protocol B: y holds the normalised rows
+    if (decode) {
+      RC(logits_from_y(y, m_y, R));
+    } else {
+      gather_rows_bf16_kernel<<<R, 128, 0, st>>>(y, d_last_rows, ylast, M.hidden);
+      LLMLB_LAUNCH_CHECK();
+      RC(logits_from_y(ylast, m_ylast, R));
+    }
+  } else if (fs->pending) {   // tp, protocol A, decode: the lm_head GEMV's prologue consumes the last down projection's collective
+    const int rc = gemv_tp_consume(tpc, fs->pending_coll, lm_head, fs->xres, fs->xother, final_norm, M.rms_eps, logits_dst(), R,
+                                   vocab_l, M.hidden, LLMLB_EPI_STORE_F32, vocab_l, tp_ll, tp_gather, st);
+    if (rc == LLMLB_E_UNSUPPORTED) {   // odd shape: fold with its own kernel, then the plain lm_head
+      RC(finish_small_tp(fs, R));
+      RC(logits_from_x(fs->xres, R));
+    } else {
+      RC(rc);
+    }
+  } else if (decode) {
+    RC(logits_from_x(fs->xres, R));
+  } else {
+    gather_rows_kernel<<<R, 256, 0, st>>>(fs->xres, d_last_rows, x_last, M.hidden);
     LLMLB_LAUNCH_CHECK();
-    return logits_from_y(ylast, m_ylast, R);
+    RC(logits_from_x(x_last, R));
   }
-  if (decode) {
-    if (fs->pending) return logits_tp_consume(fs, R);
-    return logits_from_x(fs->xres, R);
-  }
-  return LLMLB_E_INTERNAL;   // prefill with fp32 residual: run_prefill gathers the rows itself
+  if (tp == 1) return LLMLB_OK;
+  return ar_allgather_cols(tpc, logits_slot_off, logits, R, vocab_l, st);   // vocabulary slices -> full rows
 }
 
-int llmlb_engine::penalize_rows(uint32_t R) {
-  return penalize_launch(logits, R, M.vocab, pen_counts, M.vocab, S.pen_freq, S.pen_pres, pen_bias_ids, pen_bias_vals,
-                         S.pen_n_bias, LLMLB_MAX_LOGIT_BIAS, B.slots, st);
-}
-int llmlb_engine::count_sampled(uint32_t R) {
-  return penalty_count_launch(pen_counts, M.vocab, S.pen_freq, S.pen_pres, S.pen_n_bias, B.slots, B.out_ids, R, st);
-}
-int llmlb_engine::logprob_rows(uint32_t R) {
-  return logprob_launch(logits, R, M.vocab, B.out_ids, S.lp_top, B.slots, d_lp, st);
+// After the logits of R rows of B (slots in B.slots): penalties, the sampler, the logprob records, the slots' next input
+// token, the penalised rows' token counts.  pen: some row is penalised, lp: some row reports logprobs (a step with
+// neither launches exactly what it did without penalties and logprobs).
+int llmlb_engine::sample_rows(uint32_t R, bool pen, bool lp) {
+  if (pen)
+    RC(penalize_launch(logits, R, M.vocab, pen_counts, M.vocab, S.pen_freq, S.pen_pres, pen_bias_ids, pen_bias_vals,
+                       S.pen_n_bias, LLMLB_MAX_LOGIT_BIAS, B.slots, st));
+  RC(llmlb_op_sample(logits, R, M.vocab, B.temperature, B.top_p, B.top_k, B.seed, B.step, B.out_ids, st));
+  if (lp) RC(logprob_launch(logits, R, M.vocab, B.out_ids, S.lp_top, B.slots, d_lp, st));
+  step_finish_kernel<<<ceil_div(R, 128), 128, 0, st>>>(S, B, R);
+  LLMLB_LAUNCH_CHECK();
+  if (pen) RC(penalty_count_launch(pen_counts, M.vocab, S.pen_freq, S.pen_pres, S.pen_n_bias, B.slots, B.out_ids, R, st));
+  return LLMLB_OK;
 }
 
-// pen: some sequence of the batch is penalised, lp: some sequence reports logprobs (a step with neither launches
-// exactly what it did without penalties and logprobs)
-int llmlb_engine::layer_stack_decode(uint32_t nb, bool pen, bool lp) {
+// one new token per sequence in B.slots[0..nb)
+int llmlb_engine::decode_logits(uint32_t nb) {
   decode_prepare_kernel<<<ceil_div(nb, 128), 128, 0, st>>>(S, B, nb);
   LLMLB_LAUNCH_CHECK();
   RC(llmlb_op_embed(embed, B.ids, x, nb, M.hidden, M.vocab, st));
   FwdState fs;
   RC(forward_tokens(nb, true, nb, 0, &fs));
-  RC(logits_after_forward(&fs, nb, true));
-  if (pen) RC(penalize_rows(nb));
-  RC(llmlb_op_sample(logits, nb, M.vocab, B.temperature, B.top_p, B.top_k, B.seed, B.step, B.out_ids, st));
-  if (lp) RC(logprob_rows(nb));
-  step_finish_kernel<<<ceil_div(nb, 128), 128, 0, st>>>(S, B, nb);
-  LLMLB_LAUNCH_CHECK();
-  if (pen) RC(count_sampled(nb));
-  return LLMLB_OK;
+  return step_logits(&fs, nb, true);
+}
+int llmlb_engine::layer_stack_decode(uint32_t nb, bool pen, bool lp) {
+  RC(decode_logits(nb));
+  return sample_rows(nb, pen, lp);
 }
 
 int llmlb_engine::launch_decode_step(uint32_t nb, bool pen, bool lp) {
@@ -1116,6 +1116,17 @@ cudaEvent_t llmlb_engine::get_event() {
   return e;
 }
 
+int llmlb_engine::copy_out(InflightStep* step, uint32_t R, bool lp) {
+  const uint64_t ring = (out_seq++) % kRing;
+  step->host_ids = h_out[ring];
+  LLMLB_CUDA_CHECK(cudaMemcpyAsync(h_out[ring], B.out_ids, R * 4, cudaMemcpyDeviceToHost, st));
+  if (lp) {
+    step->host_lp = h_lp[ring];
+    LLMLB_CUDA_CHECK(cudaMemcpyAsync(h_lp[ring], d_lp, R * sizeof(llmlb_token_logprobs), cudaMemcpyDeviceToHost, st));
+  }
+  return LLMLB_OK;
+}
+
 // reqs[i] contributes take[i] prompt tokens starting at reqs[i]->prefilled
 int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector<uint32_t>& take) {
   uint32_t T = 0;
@@ -1164,13 +1175,7 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
       s_pos[row + j] = int32_t(pos);
       s_page[row + j] = r.pages[pos / kPageTokens];
     }
-    for (uint32_t j = 0; j < take[i]; j += pf_tile) {
-      s_tiles[n_tiles * 4 + 0] = int32_t(row + j);
-      s_tiles[n_tiles * 4 + 1] = int32_t(std::min<uint32_t>(pf_tile, take[i] - j));
-      s_tiles[n_tiles * 4 + 2] = int32_t(p0 + j);
-      s_tiles[n_tiles * 4 + 3] = r.slot;
-      ++n_tiles;
-    }
+    n_tiles = add_tiles(s_tiles, n_tiles, row, take[i], p0, r.slot);
     if (p0 + take[i] == r.prompt.size()) {
       s_rows[R] = int32_t(row + take[i] - 1);
       s_slots[R] = r.slot;
@@ -1199,32 +1204,15 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
   RC(llmlb_op_embed(embed, d_ids, x, T, M.hidden, M.vocab, st));
   FwdState fs;
   RC(forward_tokens(T, false, 0, n_tiles, &fs));
-  if (!fs.y_final) RC(finish_small_tp(&fs, T));   // tp, T <= 4: every rank folds the last collective (also when R == 0)
+  RC(finish_small_tp(&fs, T));   // tp, T <= 4: every rank folds the last collective (also when R == 0)
   if (R) {
-    if (fs.y_final) {
-      RC(logits_after_forward(&fs, R, false));
-    } else {
-      gather_rows_kernel<<<R, 256, 0, st>>>(fs.xres, d_last_rows, x_last, M.hidden);
-      LLMLB_LAUNCH_CHECK();
-      RC(logits_from_x(x_last, R));
-    }
+    RC(step_logits(&fs, R, false));
     sample_prepare_kernel<<<ceil_div(R, 128), 128, 0, st>>>(S, B, R);
     LLMLB_LAUNCH_CHECK();
-    if (pen_rows) RC(penalize_rows(R));
-    RC(llmlb_op_sample(logits, R, M.vocab, B.temperature, B.top_p, B.top_k, B.seed, B.step, B.out_ids, st));
-    if (lp_rows) RC(logprob_rows(R));
-    step_finish_kernel<<<ceil_div(R, 128), 128, 0, st>>>(S, B, R);
-    LLMLB_LAUNCH_CHECK();
-    if (pen_rows) RC(count_sampled(R));
+    RC(sample_rows(R, pen_rows, lp_rows));
     prefill_finish_kernel<<<ceil_div(R, 128), 128, 0, st>>>(S, B, R);
     LLMLB_LAUNCH_CHECK();
-    const uint64_t ring = (out_seq++) % kRing;
-    step.host_ids = h_out[ring];
-    LLMLB_CUDA_CHECK(cudaMemcpyAsync(step.host_ids, B.out_ids, R * 4, cudaMemcpyDeviceToHost, st));
-    if (lp_rows) {
-      step.host_lp = h_lp[ring];
-      LLMLB_CUDA_CHECK(cudaMemcpyAsync(h_lp[ring], d_lp, R * sizeof(llmlb_token_logprobs), cudaMemcpyDeviceToHost, st));
-    }
+    RC(copy_out(&step, R, lp_rows));
   }
   LLMLB_CUDA_CHECK(cudaEventRecord(step.ev_end, st));
   {
@@ -1278,13 +1266,7 @@ int llmlb_engine::run_decode(const std::vector<ReqPtr>& batch) {
   bool pen = false, lp = false;
   for (auto& r : batch) { pen |= r->penalized; lp |= r->top_logprobs >= 0; }
   RC(launch_decode_step(nb, pen, lp));
-  const uint64_t ring = (out_seq++) % kRing;
-  step.host_ids = h_out[ring];
-  LLMLB_CUDA_CHECK(cudaMemcpyAsync(step.host_ids, B.out_ids, nb * 4, cudaMemcpyDeviceToHost, st));
-  if (lp) {
-    step.host_lp = h_lp[ring];
-    LLMLB_CUDA_CHECK(cudaMemcpyAsync(h_lp[ring], d_lp, nb * sizeof(llmlb_token_logprobs), cudaMemcpyDeviceToHost, st));
-  }
+  RC(copy_out(&step, nb, lp));
   LLMLB_CUDA_CHECK(cudaEventRecord(step.ev_end, st));
   {
     std::lock_guard<std::mutex> lk(mu);
@@ -2130,37 +2112,34 @@ extern "C" int llmlb_debug_prefill_logits(llmlb_engine* e, const int32_t* prompt
   RC(debug_acquire(e));
   cudaStream_t st = e->st;
   const int slot = e->debug_slot;
-  std::vector<int32_t> pos(n), page(n), tiles;
+  const int32_t len = int32_t(n);
+  const uint32_t chunk = e->cfg.max_seqs;   // the rows d_last_rows (and x_last, ylast) hold
+  std::vector<int32_t> pos(n), page(n), tiles(size_t(ceil_div(n, e->pf_tile)) * 4), rows(std::min(n, chunk));
   for (uint32_t i = 0; i < n; ++i) { pos[i] = int32_t(i); page[i] = e->debug_pages[i / kPageTokens]; }
-  for (uint32_t j = 0; j < n; j += e->pf_tile) { tiles.push_back(int32_t(j)); tiles.push_back(int32_t(std::min<uint32_t>(e->pf_tile, n - j))); tiles.push_back(int32_t(j)); tiles.push_back(slot); }
-  LLMLB_CUDA_CHECK(cudaMemcpy(e->d_block_tables + size_t(slot) * e->pages_per_seq, e->debug_pages.data(), e->debug_pages.size() * 4, cudaMemcpyHostToDevice));
-  LLMLB_CUDA_CHECK(cudaMemcpy(e->d_ids, prompt, n * 4, cudaMemcpyHostToDevice));
-  LLMLB_CUDA_CHECK(cudaMemcpy(e->d_pos, pos.data(), n * 4, cudaMemcpyHostToDevice));
-  LLMLB_CUDA_CHECK(cudaMemcpy(e->d_page_of_tok, page.data(), n * 4, cudaMemcpyHostToDevice));
-  LLMLB_CUDA_CHECK(cudaMemcpy(e->d_tiles, tiles.data(), tiles.size() * 4, cudaMemcpyHostToDevice));
+  const uint32_t n_tiles = e->add_tiles(tiles.data(), 0, 0, n, 0, slot);
+  LLMLB_CUDA_CHECK(cudaMemcpyAsync(e->d_block_tables + size_t(slot) * e->pages_per_seq, e->debug_pages.data(), e->debug_pages.size() * 4,
+                                   cudaMemcpyHostToDevice, st));
+  LLMLB_CUDA_CHECK(cudaMemcpyAsync(e->d_ids, prompt, n * 4, cudaMemcpyHostToDevice, st));
+  LLMLB_CUDA_CHECK(cudaMemcpyAsync(e->d_pos, pos.data(), n * 4, cudaMemcpyHostToDevice, st));
+  LLMLB_CUDA_CHECK(cudaMemcpyAsync(e->d_page_of_tok, page.data(), n * 4, cudaMemcpyHostToDevice, st));
+  LLMLB_CUDA_CHECK(cudaMemcpyAsync(e->d_tiles, tiles.data(), tiles.size() * 4, cudaMemcpyHostToDevice, st));
   slot_init_kernel<<<1, 1, 0, st>>>(e->S, slot, 0.f, 1.f, 0, 0, 0, -1);
   LLMLB_LAUNCH_CHECK();
+  LLMLB_CUDA_CHECK(cudaMemcpyAsync(e->S.seq_len + slot, &len, 4, cudaMemcpyHostToDevice, st));   // read by the next decode step only
   RC(llmlb_op_embed(e->embed, e->d_ids, e->x, n, e->M.hidden, e->M.vocab, st));
   llmlb_engine::FwdState fs;
-  RC(e->forward_tokens(n, false, 0, (uint32_t)tiles.size() / 4, &fs));
-  if (!fs.y_final) RC(e->finish_small_tp(&fs, n));
-  const uint32_t chunk = e->cfg.max_seqs;
-  const size_t H = e->M.hidden, V = e->M.vocab;
+  RC(e->forward_tokens(n, false, 0, n_tiles, &fs));
+  RC(e->finish_small_tp(&fs, n));
+  const size_t V = e->M.vocab;
   for (uint32_t c0 = logits_all ? 0 : n - 1; c0 < n; c0 += chunk) {
-    uint32_t R = std::min(chunk, n - c0);
-    if (fs.y_final) {   // tensor parallel, protocol B: the rows are already normalised (bf16)
-      LLMLB_CUDA_CHECK(cudaMemcpyAsync(e->ylast, e->y + size_t(c0) * H, size_t(R) * H * 2, cudaMemcpyDeviceToDevice, st));
-      RC(e->logits_from_y(e->ylast, e->m_ylast, R));
-    } else {
-      LLMLB_CUDA_CHECK(cudaMemcpyAsync(e->x_last, fs.xres + size_t(c0) * H, size_t(R) * H * 4, cudaMemcpyDeviceToDevice, st));
-      RC(e->logits_from_x(e->x_last, R));
-    }
+    const uint32_t R = std::min(chunk, n - c0);
+    for (uint32_t r = 0; r < R; ++r) rows[r] = int32_t(c0 + r);
+    LLMLB_CUDA_CHECK(cudaMemcpyAsync(e->d_last_rows, rows.data(), R * 4, cudaMemcpyHostToDevice, st));
+    RC(e->step_logits(&fs, R, false));
     LLMLB_CUDA_CHECK(cudaStreamSynchronize(st));
     if (logits_all) LLMLB_CUDA_CHECK(cudaMemcpy(logits_all + size_t(c0) * V, e->logits, size_t(R) * V * 4, cudaMemcpyDeviceToHost));
     if (c0 + R == n) LLMLB_CUDA_CHECK(cudaMemcpy(logits_last, e->logits + size_t(R - 1) * V, V * 4, cudaMemcpyDeviceToHost));
   }
-  int32_t len = int32_t(n);
-  LLMLB_CUDA_CHECK(cudaMemcpy(e->S.seq_len + slot, &len, 4, cudaMemcpyHostToDevice));
   e->debug_len = n;
   e->cur_batch_slots.clear();
   return LLMLB_OK;
@@ -2174,15 +2153,10 @@ extern "C" int llmlb_debug_decode_logits(llmlb_engine* e, int32_t token, float* 
   if (e->debug_len + 1 > e->cfg.max_ctx) { set_error("context full"); return LLMLB_E_INVALID_ARG; }
   cudaStream_t st = e->st;
   int32_t slot = e->debug_slot;
-  LLMLB_CUDA_CHECK(cudaMemcpy(e->S.last_token + slot, &token, 4, cudaMemcpyHostToDevice));
-  LLMLB_CUDA_CHECK(cudaMemcpy(e->B.slots, &slot, 4, cudaMemcpyHostToDevice));
+  LLMLB_CUDA_CHECK(cudaMemcpyAsync(e->S.last_token + slot, &token, 4, cudaMemcpyHostToDevice, st));
+  LLMLB_CUDA_CHECK(cudaMemcpyAsync(e->B.slots, &slot, 4, cudaMemcpyHostToDevice, st));
   e->cur_batch_slots.clear();
-  decode_prepare_kernel<<<1, 128, 0, st>>>(e->S, e->B, 1);
-  LLMLB_LAUNCH_CHECK();
-  RC(llmlb_op_embed(e->embed, e->B.ids, e->x, 1, e->M.hidden, e->M.vocab, st));
-  llmlb_engine::FwdState fs;
-  RC(e->forward_tokens(1, true, 1, 0, &fs));
-  RC(e->logits_after_forward(&fs, 1, true));
+  RC(e->decode_logits(1));
   LLMLB_CUDA_CHECK(cudaStreamSynchronize(st));
   LLMLB_CUDA_CHECK(cudaMemcpy(logits_out, e->logits, size_t(e->M.vocab) * 4, cudaMemcpyDeviceToHost));
   e->debug_len += 1;
