@@ -169,6 +169,8 @@ extern "C" {
     pub fn llmlb_request_submit_logprobs(e: *mut llmlb_engine, prompt_ids: *const i32, n_prompt: u32, s: *const llmlb_sampling, pen: *const llmlb_penalties, top_logprobs: u32, req_id: *mut u64) -> c_int;
     pub fn llmlb_request_poll(e: *mut llmlb_engine, req_id: u64, out: *mut llmlb_token_event, cap: u32, n_out: *mut u32, timeout_ms: c_int) -> c_int;
     pub fn llmlb_request_poll_logprobs(e: *mut llmlb_engine, req_id: u64, out: *mut llmlb_token_event, lp: *mut llmlb_token_logprobs, cap: u32, n_out: *mut u32, timeout_ms: c_int) -> c_int;
+    pub fn llmlb_request_submit_prompt_logprobs(e: *mut llmlb_engine, prompt_ids: *const i32, n_prompt: u32, s: *const llmlb_sampling, pen: *const llmlb_penalties, top_logprobs: u32, req_id: *mut u64) -> c_int;
+    pub fn llmlb_request_poll_prompt_logprobs(e: *mut llmlb_engine, req_id: u64, out: *mut llmlb_token_logprobs, cap: u32, n_out: *mut u32) -> c_int;
     pub fn llmlb_request_cancel(e: *mut llmlb_engine, req_id: u64) -> c_int;
     pub fn llmlb_request_release(e: *mut llmlb_engine, req_id: u64) -> c_int;
 }

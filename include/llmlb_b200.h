@@ -225,6 +225,19 @@ int llmlb_request_submit_logprobs(llmlb_engine* e, const int32_t* prompt_ids, ui
  * submitted without logprobs, and for an event with token_id < 0, lp[i] has logprob = NaN and n_top = 0. */
 int llmlb_request_poll_logprobs(llmlb_engine* e, uint64_t req_id, llmlb_token_event* out, llmlb_token_logprobs* lp,
                                 uint32_t cap, uint32_t* n_out, int timeout_ms);
+/* Prompt logprobs (OpenAI completions' echo with logprobs; scoring a text).  For a prompt t_0 .. t_{n-1}, prompt record i
+ * (i = 0 .. n-2) reports token t_{i+1}: the arithmetic and top-n rule above, on z = the lm_head logits at position i (the
+ * row llmlb_debug_prefill_logits returns for position i), with NO penalties and NO logit bias (they control generated
+ * tokens), and top_logprobs alternatives.  t_0 has no record.  The generated tokens' records are those of
+ * llmlb_request_submit_logprobs, unchanged.
+ * llmlb_request_submit_logprobs that also computes the prompt records; top_logprobs > 20 returns LLMLB_E_INVALID_ARG. */
+int llmlb_request_submit_prompt_logprobs(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt, const llmlb_sampling* s,
+                                         const llmlb_penalties* pen, uint32_t top_logprobs, uint64_t* req_id);
+/* Non-blocking: drains up to cap prompt records computed so far, in position order.  All of a request's records are
+ * there before its first token event.  A request that ends before its prefill completes delivers fewer than n-1; a request
+ * submitted otherwise delivers none; an unknown id returns LLMLB_E_NOT_FOUND. */
+int llmlb_request_poll_prompt_logprobs(llmlb_engine* e, uint64_t req_id, llmlb_token_logprobs* out, uint32_t cap,
+                                       uint32_t* n_out);
 /* Drain up to cap events. timeout_ms: 0 = return at once, <0 = wait until at least one. */
 int llmlb_request_poll(llmlb_engine* e, uint64_t req_id, llmlb_token_event* out, uint32_t cap,
                        uint32_t* n_out, int timeout_ms);

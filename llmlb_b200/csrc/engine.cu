@@ -195,6 +195,8 @@ struct Request {
   std::vector<int32_t> bias_ids;
   std::vector<float> bias_vals;
   int32_t top_logprobs = -1;   // logprobs with this many alternatives (0..20), -1 = none (logprob.cu)
+  bool prompt_lp = false;       // also the prompt records: one per prompt position 0..n_prompt0-2, with top_logprobs alternatives
+  uint32_t prompt_lp_done = 0;  // prompt records already harvested (positions 0..prompt_lp_done-1)
   int slot = -1;
   std::vector<int32_t> pages;
   uint32_t prefilled = 0;   // context tokens whose KV is (being) written
@@ -215,6 +217,7 @@ struct Request {
   uint32_t finish_reason = LLMLB_FINISH_NONE;
   std::deque<llmlb_token_event> events;
   std::deque<llmlb_token_logprobs> lp_events;   // logprob requests: one per entry of `events`
+  std::deque<llmlb_token_logprobs> prompt_lp_events;   // prompt records not yet polled, in position order
   std::chrono::steady_clock::time_point t_submit;
 };
 using ReqPtr = std::shared_ptr<Request>;
@@ -224,6 +227,9 @@ struct InflightStep {
   int32_t* host_ids = nullptr;        // pinned
   const llmlb_token_logprobs* host_lp = nullptr;   // pinned; set when some row of the step reports logprobs
   std::vector<ReqPtr> reqs;           // batch position -> request
+  struct PromptRecords { ReqPtr r; uint32_t p0, n, off; };   // r's prompt records of positions p0..p0+n at host_plp[off..]
+  std::vector<PromptRecords> prompt_lp;
+  const llmlb_token_logprobs* host_plp = nullptr;   // pinned; set when the step computes prompt records
   bool is_prefill = false;
   uint32_t n_tokens = 0;
 };
@@ -403,13 +409,19 @@ struct llmlb_engine {
   float* pen_bias_vals = nullptr;
   int32_t* pen_gen = nullptr;
   llmlb_token_logprobs* d_lp = nullptr;   // logprob records of the step's rows [max_seqs]
+  // prompt logprobs of a prefill step: rows | target tokens | alternatives [t_cap each], and the records [t_cap]
+  int32_t* d_plp_rows = nullptr;
+  llmlb_token_logprobs* d_plp = nullptr;
   static constexpr int kRing = 8;
   uint8_t* h_stage[kRing] = {};
   size_t stage_bytes = 0;
   uint64_t stage_seq = 0;
   int32_t* h_out[kRing] = {};
   llmlb_token_logprobs* h_lp[kRing] = {};   // beside h_out[i]: the records of logprob steps
-  uint64_t out_seq = 0;
+  // the prompt records of prefill steps [t_cap], allocated at the first such step: lookahead + 1 slots, the most steps in
+  // flight at once
+  llmlb_token_logprobs* h_plp[kRing] = {};
+  uint64_t out_seq = 0, plp_seq = 0;
   std::vector<cudaEvent_t> ev_pool;
 
   // TP exchange (tp_common.cuh): one IPC-shared region per rank
@@ -490,7 +502,7 @@ struct llmlb_engine {
   int finish_small_tp(FwdState* fs, uint32_t T);                     // fold a pending collective: xres complete
   int logits_from_x(const float* src, uint32_t R);                   // fp32 rows, final norm applied here
   int logits_from_y(const __nv_bfloat16* src, const CUtensorMap* maps, uint32_t R);   // rows already normalised
-  int step_logits(FwdState* fs, uint32_t R, bool decode);            // rows 0..R (decode) or the rows in d_last_rows
+  int step_logits(FwdState* fs, uint32_t R, const int32_t* rows);    // rows 0..R of a decode step (rows NULL) or rows[0..R)
   float* logits_dst() { return tp == 1 ? logits : reinterpret_cast<float*>(xchg + logits_slot_off); }
   // prefill-attention tiles of `take` rows from `row` on, holding positions p0.. of the sequence in `slot`
   uint32_t add_tiles(int32_t* tiles, uint32_t n_tiles, uint32_t row, uint32_t take, uint32_t p0, int32_t slot) const {
@@ -733,11 +745,13 @@ int llmlb_engine::alloc_all() {
   RC(dmalloc(&pen_bias_ids, ms * LLMLB_MAX_LOGIT_BIAS)); RC(dmalloc(&pen_bias_vals, ms * LLMLB_MAX_LOGIT_BIAS));
   RC(dmalloc(&pen_gen, cfg.max_ctx));
   RC(dmalloc(&S.lp_top, ms)); RC(dmalloc(&d_lp, ms));
+  RC(dmalloc(&d_plp_rows, size_t(t_cap) * 3)); RC(dmalloc(&d_plp, t_cap));
   RC(dmalloc(&B.slots, ms)); RC(dmalloc(&B.ids, ms)); RC(dmalloc(&B.seq_lens, ms));
   RC(dmalloc(&B.temperature, ms)); RC(dmalloc(&B.top_p, ms)); RC(dmalloc(&B.top_k, ms));
   RC(dmalloc(&B.seed, ms)); RC(dmalloc(&B.step, ms)); RC(dmalloc(&B.out_ids, ms));
-  // run_prefill's layout: ids, positions, pages [t_cap each] | tiles [tiles_cap x 4] | rows, slots, lens [max_seqs each]
-  stage_bytes = size_t(t_cap) * 4 * 3 + size_t(t_cap / 64 + ms + 1) * 16 + ms * 4 * 3 + 256;
+  // run_prefill's layout: ids, positions, pages [t_cap each] | tiles [tiles_cap x 4] | rows, slots, lens [max_seqs each] |
+  // prompt-record rows, targets, alternatives [t_cap each]
+  stage_bytes = size_t(t_cap) * 4 * 3 + size_t(t_cap / 64 + ms + 1) * 16 + ms * 4 * 3 + size_t(t_cap) * 4 * 3 + 256;
   for (int i = 0; i < kRing; ++i) {
     LLMLB_CUDA_CHECK(cudaHostAlloc((void**)&h_stage[i], stage_bytes, cudaHostAllocDefault));
     LLMLB_CUDA_CHECK(cudaHostAlloc((void**)&h_out[i], ms * 4, cudaHostAllocDefault));
@@ -994,14 +1008,15 @@ int llmlb_engine::logits_from_y(const __nv_bfloat16* src, const CUtensorMap* map
   if (R <= 4) return llmlb_op_gemv(lm_head, src, nullptr, M.rms_eps, dst, R, vocab_l, H, LLMLB_EPI_STORE_F32, vocab_l, st);
   return gemm_tc_launch(m_lm_head, maps[bn_index(tc_pick_bn(R))], dst, R, vocab_l, H, LLMLB_EPI_STORE_F32, vocab_l, st, &maps[bn_index(128)]);
 }
-// logits[r, :] of the step's final hidden rows: rows 0..R of a decode step, else the R rows listed in d_last_rows (a
-// prefill has folded its last protocol-A collective already: finish_small_tp)
-int llmlb_engine::step_logits(FwdState* fs, uint32_t R, bool decode) {
+// logits[r, :] of the step's final hidden rows: rows 0..R of a decode step (rows NULL), else the R rows listed in the
+// device array `rows` (a prefill has folded its last protocol-A collective already: finish_small_tp)
+int llmlb_engine::step_logits(FwdState* fs, uint32_t R, const int32_t* rows) {
+  const bool decode = rows == nullptr;
   if (fs->y_final) {   // tp, protocol B: y holds the normalised rows
     if (decode) {
       RC(logits_from_y(y, m_y, R));
     } else {
-      gather_rows_bf16_kernel<<<R, 128, 0, st>>>(y, d_last_rows, ylast, M.hidden);
+      gather_rows_bf16_kernel<<<R, 128, 0, st>>>(y, rows, ylast, M.hidden);
       LLMLB_LAUNCH_CHECK();
       RC(logits_from_y(ylast, m_ylast, R));
     }
@@ -1017,7 +1032,7 @@ int llmlb_engine::step_logits(FwdState* fs, uint32_t R, bool decode) {
   } else if (decode) {
     RC(logits_from_x(fs->xres, R));
   } else {
-    gather_rows_kernel<<<R, 256, 0, st>>>(fs->xres, d_last_rows, x_last, M.hidden);
+    gather_rows_kernel<<<R, 256, 0, st>>>(fs->xres, rows, x_last, M.hidden);
     LLMLB_LAUNCH_CHECK();
     RC(logits_from_x(x_last, R));
   }
@@ -1047,7 +1062,7 @@ int llmlb_engine::decode_logits(uint32_t nb) {
   RC(llmlb_op_embed(embed, B.ids, x, nb, M.hidden, M.vocab, st));
   FwdState fs;
   RC(forward_tokens(nb, true, nb, 0, &fs));
-  return step_logits(&fs, nb, true);
+  return step_logits(&fs, nb, nullptr);
 }
 int llmlb_engine::layer_stack_decode(uint32_t nb, bool pen, bool lp) {
   RC(decode_logits(nb));
@@ -1141,11 +1156,12 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
   int32_t* s_rows = s_tiles + size_t(tiles_cap) * 4;
   int32_t* s_slots = s_rows + cfg.max_seqs;
   int32_t* s_lens = s_slots + cfg.max_seqs;
+  int32_t* s_plp = s_lens + cfg.max_seqs;   // prompt records: rows | targets | alternatives, t_cap apart (as d_plp_rows)
 
   InflightStep step;
   step.is_prefill = true;
   step.n_tokens = T;
-  uint32_t row = 0, n_tiles = 0, R = 0;
+  uint32_t row = 0, n_tiles = 0, R = 0, n_plp = 0;
   bool pen_rows = false;   // some finished row is penalised
   bool lp_rows = false;    // some finished row reports logprobs
   for (size_t i = 0; i < reqs.size(); ++i) {
@@ -1176,6 +1192,17 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
       s_page[row + j] = r.pages[pos / kPageTokens];
     }
     n_tiles = add_tiles(s_tiles, n_tiles, row, take[i], p0, r.slot);
+    if (r.prompt_lp) {
+      // the chunk's positions that have a next prompt token and were not reported before a preemption (which happens with
+      // nothing in flight, so prompt_lp_done is exact then; within one admission the chunks are disjoint)
+      const uint32_t lo = std::max(p0, r.prompt_lp_done), hi = std::min(p0 + take[i], r.n_prompt0 - 1);
+      if (lo < hi) step.prompt_lp.push_back({reqs[i], lo, hi - lo, n_plp});
+      for (uint32_t p = lo; p < hi; ++p, ++n_plp) {
+        s_plp[n_plp] = int32_t(row + p - p0);
+        s_plp[t_cap + n_plp] = r.prompt[p + 1];   // the target of a chunk's last row lies in the next chunk
+        s_plp[2 * t_cap + n_plp] = r.top_logprobs;
+      }
+    }
     if (p0 + take[i] == r.prompt.size()) {
       s_rows[R] = int32_t(row + take[i] - 1);
       s_slots[R] = r.slot;
@@ -1198,6 +1225,8 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
     LLMLB_CUDA_CHECK(cudaMemcpyAsync(B.seq_lens, s_lens, R * 4, cudaMemcpyHostToDevice, st));
     cur_batch_slots.clear();  // B.slots no longer holds a decode batch
   }
+  for (uint32_t k = 0; n_plp && k < 3; ++k)
+    LLMLB_CUDA_CHECK(cudaMemcpyAsync(d_plp_rows + size_t(k) * t_cap, s_plp + size_t(k) * t_cap, n_plp * 4, cudaMemcpyHostToDevice, st));
   step.ev_start = get_event();
   step.ev_end = get_event();
   LLMLB_CUDA_CHECK(cudaEventRecord(step.ev_start, st));
@@ -1206,13 +1235,32 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
   RC(forward_tokens(T, false, 0, n_tiles, &fs));
   RC(finish_small_tp(&fs, T));   // tp, T <= 4: every rank folds the last collective (also when R == 0)
   if (R) {
-    RC(step_logits(&fs, R, false));
+    RC(step_logits(&fs, R, d_last_rows));
     sample_prepare_kernel<<<ceil_div(R, 128), 128, 0, st>>>(S, B, R);
     LLMLB_LAUNCH_CHECK();
     RC(sample_rows(R, pen_rows, lp_rows));
     prefill_finish_kernel<<<ceil_div(R, 128), 128, 0, st>>>(S, B, R);
     LLMLB_LAUNCH_CHECK();
     RC(copy_out(&step, R, lp_rows));
+  }
+  // prompt records: the same lm_head path and logprob_kernel over the prompt rows, max_seqs rows at a time (the rows the
+  // logits buffers hold); no penalties or bias: those act on generated tokens
+  for (uint32_t g = 0; g < n_plp; g += cfg.max_seqs) {
+    const uint32_t G = std::min(cfg.max_seqs, n_plp - g);
+    // tp > 1: this rank's lm_head rewrites its logits exchange slot, which the peers pull in the all-gather before it (the
+    // sampled rows' or the previous group's) and which has no barrier at its end; an empty pull barrier holds the write
+    // until every peer has finished that all-gather
+    if (tp > 1) RC(ar_allreduce_add(tpc, logits_slot_off, nullptr, 0, st));
+    RC(step_logits(&fs, G, d_plp_rows + g));
+    RC(logprob_launch(logits, G, M.vocab, d_plp_rows + t_cap + g, d_plp_rows + 2 * t_cap + g, nullptr, d_plp + g, st));
+  }
+  if (n_plp) {
+    if (!h_plp[0])
+      for (uint32_t i = 0; i <= lookahead; ++i)
+        LLMLB_CUDA_CHECK(cudaHostAlloc((void**)&h_plp[i], size_t(t_cap) * sizeof(llmlb_token_logprobs), cudaHostAllocDefault));
+    llmlb_token_logprobs* dst = h_plp[(plp_seq++) % (lookahead + 1)];
+    step.host_plp = dst;
+    LLMLB_CUDA_CHECK(cudaMemcpyAsync(dst, d_plp, n_plp * sizeof(llmlb_token_logprobs), cudaMemcpyDeviceToHost, st));
   }
   LLMLB_CUDA_CHECK(cudaEventRecord(step.ev_end, st));
   {
@@ -1348,6 +1396,12 @@ void llmlb_engine::harvest_one() {
   if (step.is_prefill) gpu_ms_prefill += ms; else gpu_ms_decode += ms;
   ev_pool.push_back(step.ev_start);
   ev_pool.push_back(step.ev_end);
+  // prompt records first: a request's last ones come from the step that also samples its first token
+  for (const auto& pr : step.prompt_lp) {
+    if (pr.r->finished || ce != cudaSuccess) continue;   // cancelled or finished: its records are dropped
+    pr.r->prompt_lp_events.insert(pr.r->prompt_lp_events.end(), step.host_plp + pr.off, step.host_plp + pr.off + pr.n);
+    pr.r->prompt_lp_done = pr.p0 + pr.n;
+  }
   auto now = std::chrono::steady_clock::now();
   for (size_t b = 0; b < step.reqs.size(); ++b) {
     const ReqPtr& r = step.reqs[b];
@@ -1552,7 +1606,9 @@ void llmlb_engine::loop_follower() {
           r->penalized = true;
           p += size_t(n_bias) * 8;
         }
-        if (size_t(buf.data() + buf.size() - p) >= 4) memcpy(&r->top_logprobs, p, 4);   // a logprob request
+        const size_t rest = size_t(buf.data() + buf.size() - p);
+        if (rest >= 4) memcpy(&r->top_logprobs, p, 4);   // a logprob request
+        if (rest >= 8) r->prompt_lp = true;              // that also reports its prompt
         r->client_released = true;
         r->t_submit = std::chrono::steady_clock::now();
         std::lock_guard<std::mutex> lk(mu);
@@ -1643,13 +1699,14 @@ extern "C" void llmlb_engine_destroy(llmlb_engine* e) {
   F(e->d_ids); F(e->d_pos); F(e->d_page_of_tok); F(e->d_tiles); F(e->d_last_rows);
   F(e->S.seq_len); F(e->S.last_token); F(e->S.temperature); F(e->S.top_p); F(e->S.top_k); F(e->S.seed); F(e->S.step);
   F(e->S.pen_freq); F(e->S.pen_pres); F(e->S.pen_n_bias); F(e->pen_counts); F(e->pen_bias_ids); F(e->pen_bias_vals); F(e->pen_gen);
-  F(e->S.lp_top); F(e->d_lp);
+  F(e->S.lp_top); F(e->d_lp); F(e->d_plp_rows); F(e->d_plp);
   F(e->B.slots); F(e->B.ids); F(e->B.seq_lens); F(e->B.temperature); F(e->B.top_p); F(e->B.top_k);
   F(e->B.seed); F(e->B.step); F(e->B.out_ids);
   for (int i = 0; i < llmlb_engine::kRing; ++i) {
     if (e->h_stage[i]) cudaFreeHost(e->h_stage[i]);
     if (e->h_out[i]) cudaFreeHost(e->h_out[i]);
     if (e->h_lp[i]) cudaFreeHost(e->h_lp[i]);
+    if (e->h_plp[i]) cudaFreeHost(e->h_plp[i]);
   }
   if (e->tp_ready)
     for (uint32_t r = 0; r < e->tp; ++r)
@@ -1724,7 +1781,7 @@ static int take_penalties(const llmlb_penalties* pen, uint32_t vocab, Request* r
 }
 
 static int submit_request(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt, const llmlb_sampling* s,
-                          const llmlb_penalties* pen, int32_t top_logprobs, uint64_t* req_id, const char* bad_arg);
+                          const llmlb_penalties* pen, int32_t top_logprobs, bool prompt_lp, uint64_t* req_id, const char* bad_arg);
 
 extern "C" int llmlb_request_submit(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt,
                                     const llmlb_sampling* s, uint64_t* req_id) {
@@ -1733,7 +1790,7 @@ extern "C" int llmlb_request_submit(llmlb_engine* e, const int32_t* prompt_ids, 
 
 extern "C" int llmlb_request_submit_penalized(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt,
                                               const llmlb_sampling* s, const llmlb_penalties* pen, uint64_t* req_id) {
-  return submit_request(e, prompt_ids, n_prompt, s, pen, -1, req_id,
+  return submit_request(e, prompt_ids, n_prompt, s, pen, -1, false, req_id,
                         pen ? "llmlb_request_submit_penalized: bad argument" : "llmlb_request_submit: bad argument");
 }
 
@@ -1744,13 +1801,24 @@ extern "C" int llmlb_request_submit_logprobs(llmlb_engine* e, const int32_t* pro
     set_error("llmlb_request_submit_logprobs: top_logprobs must be in [0, 20]");
     return LLMLB_E_INVALID_ARG;
   }
-  return submit_request(e, prompt_ids, n_prompt, s, pen, int32_t(top_logprobs), req_id,
+  return submit_request(e, prompt_ids, n_prompt, s, pen, int32_t(top_logprobs), false, req_id,
                         "llmlb_request_submit_logprobs: bad argument");
 }
 
-// top_logprobs: -1 = the request reports no logprobs
+extern "C" int llmlb_request_submit_prompt_logprobs(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt,
+                                                    const llmlb_sampling* s, const llmlb_penalties* pen, uint32_t top_logprobs,
+                                                    uint64_t* req_id) {
+  if (top_logprobs > LLMLB_MAX_TOP_LOGPROBS) {
+    set_error("llmlb_request_submit_prompt_logprobs: top_logprobs must be in [0, 20]");
+    return LLMLB_E_INVALID_ARG;
+  }
+  return submit_request(e, prompt_ids, n_prompt, s, pen, int32_t(top_logprobs), true, req_id,
+                        "llmlb_request_submit_prompt_logprobs: bad argument");
+}
+
+// top_logprobs: -1 = the request reports no logprobs; prompt_lp (with top_logprobs >= 0): also its prompt records
 static int submit_request(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt, const llmlb_sampling* s,
-                          const llmlb_penalties* pen, int32_t top_logprobs, uint64_t* req_id, const char* bad_arg) {
+                          const llmlb_penalties* pen, int32_t top_logprobs, bool prompt_lp, uint64_t* req_id, const char* bad_arg) {
   if (!e || !prompt_ids || !s || !req_id || n_prompt == 0) {
     set_error(bad_arg);
     return LLMLB_E_INVALID_ARG;
@@ -1768,6 +1836,7 @@ static int submit_request(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n
   auto r = std::make_shared<Request>();
   RC(take_penalties(pen, e->M.vocab, r.get()));
   r->top_logprobs = top_logprobs;
+  r->prompt_lp = prompt_lp;
   r->prompt.assign(prompt_ids, prompt_ids + n_prompt);
   r->n_prompt0 = n_prompt;
   r->s = *s;
@@ -1784,11 +1853,11 @@ static int submit_request(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n
     e->requests[r->id] = r;
     e->waiting.push_back(r);
     *req_id = r->id;
-    if (e->plan_on) {   // id, sampling, prompt, stop ids, (penalised requests) the penalties and (logprob requests)
-                        // top_logprobs travel to the followers in queue order
+    if (e->plan_on) {   // id, sampling, prompt, stop ids, (penalised requests) the penalties, (logprob requests)
+                        // top_logprobs and (prompt logprobs) the prompt flag travel to the followers in queue order
       const uint32_t n_bias = uint32_t(r->bias_ids.size());
       std::vector<uint8_t> rec(8 + sizeof(llmlb_sampling) + 8 + (size_t(n_prompt) + r->stop_ids.size()) * 4 +
-                               (r->penalized ? 12 + size_t(n_bias) * 8 : 0) + (top_logprobs >= 0 ? 4 : 0));
+                               (r->penalized ? 12 + size_t(n_bias) * 8 : 0) + (top_logprobs >= 0 ? 4 : 0) + (prompt_lp ? 4 : 0));
       uint8_t* p = rec.data();
       memcpy(p, &r->id, 8); p += 8;
       memcpy(p, &r->s, sizeof(llmlb_sampling)); p += sizeof(llmlb_sampling);
@@ -1802,8 +1871,10 @@ static int submit_request(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n
         if (n_bias) { memcpy(p, r->bias_ids.data(), size_t(n_bias) * 4); memcpy(p + size_t(n_bias) * 4, r->bias_vals.data(), size_t(n_bias) * 4); }
         p += size_t(n_bias) * 8;
       }
-      // [i32 top_logprobs]: 4 bytes, so a follower cannot take it for a penalty block (at least 12)
+      // [i32 top_logprobs][u32 1 = prompt logprobs]: 4 or 8 bytes, so a follower cannot take them for a penalty block (at
+      // least 12)
       if (top_logprobs >= 0) memcpy(p, &top_logprobs, 4);
+      if (prompt_lp) { const uint32_t one = 1; memcpy(p + 4, &one, 4); }
       e->plan_log(kPlanSubmit, rec.data(), uint32_t(rec.size()));
     }
   }
@@ -1837,6 +1908,18 @@ extern "C" int llmlb_request_poll_logprobs(llmlb_engine* e, uint64_t req_id, llm
     out[(*n_out)++] = r->events.front();
     r->events.pop_front();
   }
+  return LLMLB_OK;
+}
+
+extern "C" int llmlb_request_poll_prompt_logprobs(llmlb_engine* e, uint64_t req_id, llmlb_token_logprobs* out, uint32_t cap,
+                                                  uint32_t* n_out) {
+  if (!e || !out || !n_out || cap == 0) { set_error("llmlb_request_poll_prompt_logprobs: bad argument"); return LLMLB_E_INVALID_ARG; }
+  *n_out = 0;
+  std::lock_guard<std::mutex> lk(e->mu);
+  auto it = e->requests.find(req_id);
+  if (it == e->requests.end()) { set_error("unknown request id"); return LLMLB_E_NOT_FOUND; }
+  auto& q = it->second->prompt_lp_events;
+  while (*n_out < cap && !q.empty()) { out[(*n_out)++] = q.front(); q.pop_front(); }
   return LLMLB_OK;
 }
 
@@ -2135,7 +2218,7 @@ extern "C" int llmlb_debug_prefill_logits(llmlb_engine* e, const int32_t* prompt
     const uint32_t R = std::min(chunk, n - c0);
     for (uint32_t r = 0; r < R; ++r) rows[r] = int32_t(c0 + r);
     LLMLB_CUDA_CHECK(cudaMemcpyAsync(e->d_last_rows, rows.data(), R * 4, cudaMemcpyHostToDevice, st));
-    RC(e->step_logits(&fs, R, false));
+    RC(e->step_logits(&fs, R, e->d_last_rows));
     LLMLB_CUDA_CHECK(cudaStreamSynchronize(st));
     if (logits_all) LLMLB_CUDA_CHECK(cudaMemcpy(logits_all + size_t(c0) * V, e->logits, size_t(R) * V * 4, cudaMemcpyDeviceToHost));
     if (c0 + R == n) LLMLB_CUDA_CHECK(cudaMemcpy(logits_last, e->logits + size_t(R - 1) * V, V * 4, cudaMemcpyDeviceToHost));

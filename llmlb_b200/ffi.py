@@ -95,6 +95,8 @@ PROTOTYPES = {
     "llmlb_request_submit_logprobs": (C.c_int, [vp, _P(i32), u32, _P(Sampling), _P(Penalties), u32, _P(u64)]),
     "llmlb_request_poll": (C.c_int, [vp, u64, _P(TokenEvent), u32, _P(u32), C.c_int]),
     "llmlb_request_poll_logprobs": (C.c_int, [vp, u64, _P(TokenEvent), _P(TokenLogprobs), u32, _P(u32), C.c_int]),
+    "llmlb_request_submit_prompt_logprobs": (C.c_int, [vp, _P(i32), u32, _P(Sampling), _P(Penalties), u32, _P(u64)]),
+    "llmlb_request_poll_prompt_logprobs": (C.c_int, [vp, u64, _P(TokenLogprobs), u32, _P(u32)]),
     "llmlb_request_cancel": (C.c_int, [vp, u64]),
     "llmlb_request_release": (C.c_int, [vp, u64]),
     "llmlb_debug_prefill_logits": (C.c_int, [vp, _P(i32), u32, _P(f32), _P(f32)]),
@@ -230,11 +232,16 @@ class Engine:
     # ---- requests ----
     def submit(self, prompt_ids, max_tokens, temperature=0.0, top_k=0, top_p=1.0, seed=0,
                stop_ids=(), ignore_eos=False, frequency_penalty=None, presence_penalty=None, logit_bias=None,
-               logprobs=None):
+               logprobs=None, prompt_logprobs=False):
         """frequency_penalty / presence_penalty / logit_bias ({token id: value}): OpenAI's penalties, applied on the device
         before sampling (llmlb_penalties).  Given at all (even neutral), the request goes through
         llmlb_request_submit_penalized.  logprobs (0..20 alternatives per token; None = off): the request reports
-        logprobs (llmlb_token_logprobs, read with poll_logprobs) and goes through llmlb_request_submit_logprobs."""
+        logprobs (llmlb_token_logprobs, read with poll_logprobs) and goes through llmlb_request_submit_logprobs.
+        prompt_logprobs (needs logprobs): also the prompt's records (poll_prompt_logprobs), through
+        llmlb_request_submit_prompt_logprobs."""
+        if prompt_logprobs and logprobs is None:
+            raise ValueError("prompt_logprobs needs logprobs (the number of alternatives)")
+        submit_lp = lib().llmlb_request_submit_prompt_logprobs if prompt_logprobs else lib().llmlb_request_submit_logprobs
         n = len(prompt_ids)
         arr = (i32 * n)(*prompt_ids)
         s = Sampling()
@@ -248,7 +255,7 @@ class Engine:
             if logprobs is None:
                 check(lib().llmlb_request_submit(self._h, arr, n, C.byref(s), C.byref(rid)))
             else:
-                check(lib().llmlb_request_submit_logprobs(self._h, arr, n, C.byref(s), None, int(logprobs), C.byref(rid)))
+                check(submit_lp(self._h, arr, n, C.byref(s), None, int(logprobs), C.byref(rid)))
             return rid.value
         bias = list((logit_bias or {}).items())
         ids = (i32 * max(1, len(bias)))(*[int(k) for k, _ in bias])
@@ -260,7 +267,7 @@ class Engine:
         if logprobs is None:
             check(lib().llmlb_request_submit_penalized(self._h, arr, n, C.byref(s), C.byref(pen), C.byref(rid)))
         else:
-            check(lib().llmlb_request_submit_logprobs(self._h, arr, n, C.byref(s), C.byref(pen), int(logprobs), C.byref(rid)))
+            check(submit_lp(self._h, arr, n, C.byref(s), C.byref(pen), int(logprobs), C.byref(rid)))
         return rid.value
 
     def poll(self, rid, cap=256, timeout_ms=0):
@@ -287,6 +294,14 @@ class Engine:
                      prompt_tokens=e.prompt_tokens, completion_tokens=e.completion_tokens, t_ms=e.t_ms,
                      logprob=r.logprob, top_logprobs=[(r.top_ids[i], r.top_logprobs[i]) for i in range(r.n_top)])
                 for e, r in zip(buf[:n.value], lp[:n.value])]
+
+    def poll_prompt_logprobs(self, rid, cap=256):
+        """The prompt records computed so far (non-blocking), in position order: [dict(logprob, top_logprobs)], where
+        top_logprobs is [(token id, logprob)], best first."""
+        lp = (TokenLogprobs * cap)()
+        n = u32()
+        check(lib().llmlb_request_poll_prompt_logprobs(self._h, rid, lp, cap, C.byref(n)))
+        return [dict(logprob=r.logprob, top_logprobs=[(r.top_ids[i], r.top_logprobs[i]) for i in range(r.n_top)]) for r in lp[:n.value]]
 
     def generate(self, prompt_ids, max_tokens, **kw):
         """submit + drain; returns (token ids, events).  With logprobs=, the events carry them (poll_logprobs)."""

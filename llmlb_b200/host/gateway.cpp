@@ -614,10 +614,15 @@ Json completion_logprobs(const std::vector<LogprobEntry>& entries) {
   Json tokens = Json::array(), lps = Json::array(), tops = Json::array(), offs = Json::array();
   for (const auto& e : entries) {
     tokens.push(e.tok.token);
-    lps.push(logprob_value(e.tok.logprob));
-    Json top = Json::object();   // two alternatives with the same text: the more probable one is kept
-    for (const auto& t : e.top) if (!top.get(t.token)) top.set(t.token, logprob_value(t.logprob));
-    tops.push(top);
+    if (!e.scored) {
+      lps.push(Json());
+      tops.push(Json());
+    } else {
+      lps.push(logprob_value(e.tok.logprob));
+      Json top = Json::object();   // two alternatives with the same text: the more probable one is kept
+      for (const auto& t : e.top) if (!top.get(t.token)) top.set(t.token, logprob_value(t.logprob));
+      tops.push(top);
+    }
     offs.push(Json(e.text_offset));
   }
   Json root = Json::object();

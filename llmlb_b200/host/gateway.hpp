@@ -284,6 +284,7 @@ struct LogprobEntry {
   LogprobToken tok;
   std::vector<LogprobToken> top;   // most probable first
   uint32_t text_offset = 0;        // code points of completion text released before the token was fed
+  bool scored = true;              // false: an echoed prompt's first token, which has no record (logprob and top are null)
 };
 // chat: {"content":[{"token","logprob","bytes","top_logprobs":[{"token","logprob","bytes"}]}],"refusal":null}
 Json chat_logprobs(const std::vector<LogprobEntry>& entries);

@@ -40,6 +40,8 @@
 #pragma weak llmlb_request_submit_penalized
 #pragma weak llmlb_request_submit_logprobs
 #pragma weak llmlb_request_poll_logprobs
+#pragma weak llmlb_request_submit_prompt_logprobs
+#pragma weak llmlb_request_poll_prompt_logprobs
 #include "anthropic.hpp"
 #include "checkpoint.hpp"
 #include "download.hpp"
@@ -237,6 +239,7 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
     if (n->is_number() && n->as_int() != 1) { send_err(400, "n must be 1: this endpoint returns one choice per request", "invalid_request_error"); return; }
   // prompt
   std::vector<int32_t> ids;
+  const std::string* prompt_str = nullptr;   // completions: the prompt as the client sent it, when it is a string
   if (const Json* raw = req.get("prompt_token_ids")) {
     if (raw->is_array()) for (auto& v : raw->items()) ids.push_back(int32_t(v.as_int()));
   } else if (kind == 0) {
@@ -274,6 +277,7 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
     const Json* one = p;
     if (p && p->is_array() && p->items().size() == 1 && (p->items()[0].is_string() || p->items()[0].is_array())) one = &p->items()[0];
     if (one && one->is_string()) {
+      prompt_str = &one->str();
       ids = G.tok ? G.tok->encode(one->str(), /*add_bos=*/true, /*parse_special=*/false) : byte_tokenize(one->str(), G.vocab);
     } else if (one && one->is_array() && all_ints(*one)) {
       for (auto& v : one->items()) ids.push_back(int32_t(std::max<int64_t>(-1, std::min<int64_t>(v.as_int(), INT32_MAX))));
@@ -365,8 +369,9 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
   pen.bias_values = bias_vals.data();
   pen.n_bias = uint32_t(bias_ids.size());
   // OpenAI's logprobs.  Chat: "logprobs" true / false / null and "top_logprobs" 0..20 / null (only with logprobs: true).
-  // Completions: "logprobs" 0..5 / null, the legacy limit, and not with echo (prompt logprobs are not served).
-  bool lp_on = false;
+  // Completions: "logprobs" 0..5 / null, the legacy limit; with echo the prompt tokens are listed first (prompt records).
+  const bool echo = kind == 2 && req.get("echo") && req.get("echo")->as_bool();
+  bool lp_on = false, lp_prompt = false;
   uint32_t lp_top = 0;
   if (kind == 0 && !anthropic) {
     const Json* lp = req.get("logprobs");
@@ -388,9 +393,13 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
         send_err(400, "logprobs must be an integer in [0, 5]", "invalid_request_error");
         return;
       }
-      const Json* echo = req.get("echo");
-      if (echo && echo->as_bool()) { send_err(400, "echo together with logprobs is not supported: prompt logprobs are not served", "invalid_request_error"); return; }
+      if (echo && !(llmlb_request_submit_prompt_logprobs && llmlb_request_poll_prompt_logprobs)) {
+        send_err(400, "echo together with logprobs is not supported by the engine library this server runs on: prompt logprobs are not served",
+                 "invalid_request_error");
+        return;
+      }
       lp_on = true;
+      lp_prompt = echo;
       lp_top = uint32_t(lp->as_int());
     }
   }
@@ -406,6 +415,7 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
   const auto t0 = std::chrono::steady_clock::now();
   uint64_t rid = 0;
   int rc = !s.max_tokens ? LLMLB_E_INVALID_ARG
+           : lp_prompt    ? llmlb_request_submit_prompt_logprobs(G.eng, ids.data(), uint32_t(ids.size()), &s, penalized ? &pen : nullptr, lp_top, &rid)
            : lp_on        ? llmlb_request_submit_logprobs(G.eng, ids.data(), uint32_t(ids.size()), &s, penalized ? &pen : nullptr, lp_top, &rid)
            : penalized    ? llmlb_request_submit_penalized(G.eng, ids.data(), uint32_t(ids.size()), &s, &pen, &rid)
                           : llmlb_request_submit(G.eng, ids.data(), uint32_t(ids.size()), &s, &rid);
@@ -445,10 +455,43 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
   std::string text;
   BpeTokenizer::Stream detok;
   uint32_t prompt_tokens = uint32_t(ids.size()), completion_tokens = 0, finish = LLMLB_FINISH_NONE;
+  auto code_points = [](const std::string& t) { uint32_t n = 0; for (unsigned char c : t) n += (c & 0xC0) != 0x80; return n; };
+  // echo: the choice's text starts with the prompt text — the client's string, or the ids through the streaming detokenizer
+  // (special tokens skipped, as for generated text); prompt_offs[i] = the code points of that text before prompt token i.
+  // For a string the offsets are taken in the string itself: the bytes of the string that the tokens before i were made
+  // of (the tokenizer's raw bytes of each non-special token, one byte per token of the byte-level placeholder), so they
+  // point into the text returned even where detokenizing would not give the string back.
+  std::string prompt_text;
+  std::vector<uint32_t> prompt_offs;
+  if (echo && prompt_str) {
+    prompt_text = *prompt_str;
+    size_t at = 0;
+    uint32_t cps = 0;   // code points that start before `at`
+    for (int32_t t : ids) {
+      // a character cut by a token boundary counts from the token that completes it, as the streaming detokenizer releases it
+      const bool cut = at < prompt_text.size() && (static_cast<unsigned char>(prompt_text[at]) & 0xC0) == 0x80;
+      prompt_offs.push_back(cps - (cut ? 1 : 0));
+      const size_t n = G.tok ? (G.tok->is_special(t) ? 0 : G.tok->token_bytes(t).size()) : 1;
+      const size_t end = std::min(prompt_text.size(), at + n);
+      cps += code_points(prompt_text.substr(at, end - at));
+      at = end;
+    }
+  } else if (echo) {
+    BpeTokenizer::Stream pd;
+    uint32_t cps = 0;
+    for (int32_t t : ids) {
+      prompt_offs.push_back(cps);
+      const std::string piece = G.tok ? G.tok->decode_next(&pd, t, /*skip_special=*/true) : byte_detokenize(t);
+      prompt_text += piece;
+      cps += code_points(piece);
+    }
+    if (G.tok) prompt_text += BpeTokenizer::flush(&pd);
+  }
+  bool prompt_sent = !echo;            // the prompt text (and its entries) went out: stream chunk / head of lp_all
   // logprobs: every generated token fed to the text path is listed, except the stop ids (their text is skipped)
   std::vector<LogprobEntry> lp_all;    // the whole list (response body)
   size_t lp_sent = 0;                  // entries of lp_all already streamed
-  uint32_t text_cps = 0;               // code points of `text`
+  uint32_t text_cps = echo ? code_points(prompt_text) : 0;   // code points of the echoed prompt and `text`
   auto lp_token = [&](int32_t id, float v) {
     LogprobToken t;
     t.bytes = G.tok ? G.tok->token_bytes(id) : byte_detokenize(id);
@@ -467,6 +510,32 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
     // connection and its upstream request with it; a buffered response would otherwise run to its last token for nobody
     if (!client_gone && peer_closed(fd)) { ok = false; client_gone = true; llmlb_request_cancel(G.eng, rid); }
     std::string out;
+    if (!prompt_sent && got) {   // the first event: every prompt record is queued before it
+      prompt_sent = true;
+      if (lp_prompt) {
+        std::vector<llmlb_token_logprobs> recs;
+        for (uint32_t n_rec = 64; n_rec == 64;) {
+          llmlb_token_logprobs buf[64];
+          n_rec = 0;
+          if (llmlb_request_poll_prompt_logprobs(G.eng, rid, buf, 64, &n_rec) != LLMLB_OK) break;
+          recs.insert(recs.end(), buf, buf + n_rec);
+        }
+        for (size_t k = 0; k < ids.size(); ++k) {
+          LogprobEntry e;
+          e.scored = k > 0 && k - 1 < recs.size();   // the first token has no record; one cut short by a cancel neither
+          e.tok = lp_token(ids[k], e.scored ? recs[k - 1].logprob : 0.f);
+          if (e.scored)
+            for (uint32_t j = 0; j < recs[k - 1].n_top && j < LLMLB_MAX_TOP_LOGPROBS; ++j) e.top.push_back(lp_token(recs[k - 1].top_ids[j], recs[k - 1].top_logprobs[j]));
+          e.text_offset = prompt_offs[k];
+          lp_all.push_back(std::move(e));
+        }
+      }
+      if (stream) {
+        lp_sent = lp_all.size();
+        const Json lj = lp_on ? lp_json(lp_all) : Json();
+        out += sse_event(completion_chunk(id, jm->str(), created, &prompt_text, nullptr, lp_on ? &lj : nullptr));
+      }
+    }
     for (uint32_t i = 0; i < got; ++i) {
       if (ev[i].token_id >= 0) {
         // with a tokenizer a delta only carries complete UTF-8 (a character split over tokens waits)
@@ -482,7 +551,7 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
           lp_all.push_back(std::move(e));
         }
         text += piece;
-        for (unsigned char c : piece) text_cps += (c & 0xC0) != 0x80;
+        text_cps += code_points(piece);
         if (stream && lp_on && (!piece.empty() || lp_sent < lp_all.size())) {
           // held-back text (a split character, a possible stop prefix) still sends its entries, with empty text
           const std::vector<LogprobEntry> fresh(lp_all.begin() + lp_sent, lp_all.end());
@@ -574,7 +643,7 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
     const Json* lpp = lp_on ? &lj : nullptr;
     Json body = kind == 0 ? chat_completion_body(id, jm->str(), created, text, fr, prompt_tokens, completion_tokens, lpp)
               : kind == 1 ? responses_body(id, jm->str(), created, text, prompt_tokens, completion_tokens, "completed")
-                          : completion_body(id, jm->str(), created, text, fr, prompt_tokens, completion_tokens, lpp);
+                          : completion_body(id, jm->str(), created, prompt_text + text, fr, prompt_tokens, completion_tokens, lpp);
     send_json(fd, 200, body.dump());
   }
 }
