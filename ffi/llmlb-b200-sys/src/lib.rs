@@ -72,7 +72,9 @@ pub struct llmlb_engine_config {
     pub request_timeout_ms: u32,
     pub attn_impl: u32,
     pub tp_proto: u32,
-    pub reserved: [u32; 3],
+    /// automatic prefix caching: 0 = off (the header documents the policy)
+    pub prefix_cache: u32,
+    pub reserved: [u32; 2],
 }
 
 #[repr(C)]
@@ -104,6 +106,18 @@ pub struct llmlb_health {
     pub gpu_ms_decode: f64,
     pub kernel_launches: u64,
     pub preemptions: u64,
+}
+
+/// Prefix-cache counters (`llmlb_engine_prefix_cache_stats`); all 0 with the cache off.
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct llmlb_prefix_cache_stats {
+    pub cached_pages: u32,
+    pub evictable_pages: u32,
+    pub lookups: u64,
+    pub hit_tokens: u64,
+    pub published_pages: u64,
+    pub evicted_pages: u64,
 }
 
 #[repr(C)]
@@ -158,6 +172,7 @@ extern "C" {
     pub fn llmlb_engine_destroy(e: *mut llmlb_engine);
     pub fn llmlb_engine_model_info(e: *const llmlb_engine, out: *mut llmlb_model_info) -> c_int;
     pub fn llmlb_engine_health(e: *const llmlb_engine, out: *mut llmlb_health) -> c_int;
+    pub fn llmlb_engine_prefix_cache_stats(e: *const llmlb_engine, out: *mut llmlb_prefix_cache_stats) -> c_int;
     pub fn llmlb_engine_load_tensor(e: *mut llmlb_engine, name: *const c_char, host_bf16: *const u8, rows: u64, cols: u64) -> c_int;
     pub fn llmlb_engine_set_rope_freq_factors(e: *mut llmlb_engine, factors: *const f32, n: u32) -> c_int;
     pub fn llmlb_engine_tp_export(e: *mut llmlb_engine, handle: *mut u8) -> c_int;
@@ -171,6 +186,7 @@ extern "C" {
     pub fn llmlb_request_poll_logprobs(e: *mut llmlb_engine, req_id: u64, out: *mut llmlb_token_event, lp: *mut llmlb_token_logprobs, cap: u32, n_out: *mut u32, timeout_ms: c_int) -> c_int;
     pub fn llmlb_request_submit_prompt_logprobs(e: *mut llmlb_engine, prompt_ids: *const i32, n_prompt: u32, s: *const llmlb_sampling, pen: *const llmlb_penalties, top_logprobs: u32, req_id: *mut u64) -> c_int;
     pub fn llmlb_request_poll_prompt_logprobs(e: *mut llmlb_engine, req_id: u64, out: *mut llmlb_token_logprobs, cap: u32, n_out: *mut u32) -> c_int;
+    pub fn llmlb_request_cached_tokens(e: *mut llmlb_engine, req_id: u64, n: *mut u32) -> c_int;
     pub fn llmlb_request_cancel(e: *mut llmlb_engine, req_id: u64) -> c_int;
     pub fn llmlb_request_release(e: *mut llmlb_engine, req_id: u64) -> c_int;
 }
@@ -282,7 +298,8 @@ impl Engine {
             request_timeout_ms: 120_000,
             attn_impl: 0,
             tp_proto: 0,
-            reserved: [0; 3],
+            prefix_cache: 0,
+            reserved: [0; 2],
         }
     }
 
@@ -343,6 +360,20 @@ impl Engine {
         let mut h = llmlb_health::default();
         check(unsafe { llmlb_engine_health(self.raw, &mut h) })?;
         Ok(h)
+    }
+
+    /// Prefix-cache counters (all 0 with `prefix_cache` off).
+    pub fn prefix_cache_stats(&self) -> Result<llmlb_prefix_cache_stats, EngineError> {
+        let mut st = llmlb_prefix_cache_stats::default();
+        check(unsafe { llmlb_engine_prefix_cache_stats(self.raw, &mut st) })?;
+        Ok(st)
+    }
+
+    /// OpenAI's `usage.prompt_tokens_details.cached_tokens` of a request.
+    pub fn cached_tokens(&self, req_id: u64) -> Result<u32, EngineError> {
+        let mut n = 0u32;
+        check(unsafe { llmlb_request_cached_tokens(self.raw, req_id, &mut n) })?;
+        Ok(n)
     }
 
     pub fn model_info(&self) -> Result<llmlb_model_info, EngineError> {

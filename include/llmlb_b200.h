@@ -85,7 +85,29 @@ typedef struct llmlb_engine_config {
   uint32_t attn_impl;          /* prefill attention: 0 = wgmma + TMA (default), 1 = mma.sync baseline */
   uint32_t tp_proto;           /* tensor-parallel decode exchange: bit 0: 0 = {value, epoch} pairs (default), 1 = values + flags;
                                   bit 1: 1 = owner CTAs fold the partials and the consumer grid gathers the result through L2 */
-  uint32_t reserved[3];
+  /* Automatic prefix caching (0 = off, the default).  Full 64-token KV pages outlive the request that computed them and
+   * are reused by later requests whose context starts with the same tokens:
+   *  - A cached page is keyed by its parent page (the cached page of the previous 64 positions; none for positions 0-63)
+   *    and its 64 token ids.  A lookup compares the ids exactly: a hash collision can never hand out wrong KV.
+   *  - Only full pages are shared, so no sequence ever writes into a page another sequence can read.
+   *  - At admission, a request walks the cache along its context (the prompt, plus after a preemption the tokens
+   *    generated so far).  At most floor((n_context - 1) / 64) pages match, so at least one token is prefilled; the
+   *    prefill starts after the matched pages.  Requests with prompt logprobs do not look up (every prompt row needs
+   *    its logits).
+   *  - A prefill step publishes the full pages it completes when it is launched.  A finished, cancelled or preempted
+   *    request publishes its full pages whose positions were all inputs of launched steps, generated tokens included:
+   *    chat turn N+1 hits on turn N's reply.  A page whose key is cached already goes back to the free pool.
+   *  - A cached page held by no request is evictable.  Pages are taken from the free pool first, then by evicting the
+   *    least recently released evictable page (deepest first among equals, so always a leaf); sequences are preempted
+   *    only after that.  The cache never holds a page a request could otherwise use: llmlb_health.free_kv_pages counts
+   *    free and evictable pages.
+   *  - A hit prefills a narrower step than a cold prompt, so its logits can differ from a cold run's in the last bits
+   *    (the projections' K-split depends on the step width).  A hit is bit-identical to a cold prefill chunked at the
+   *    same boundary.
+   *  - llmlb_engine_load_tensor after the first request or debug call returns LLMLB_E_UNSUPPORTED (cached KV would be
+   *    stale).  The debug hooks drop the cache.  With tensor parallelism every rank sets the same value. */
+  uint32_t prefix_cache;
+  uint32_t reserved[2];
 } llmlb_engine_config;
 
 int llmlb_engine_create(const llmlb_engine_config* cfg, llmlb_engine** out);
@@ -153,6 +175,16 @@ typedef struct llmlb_health {      /* feeds GET /api/health (endpoint_checker.rs
   uint64_t preemptions;            /* sequences evicted (pages reclaimed, recomputed later) so far */
 } llmlb_health;
 int llmlb_engine_health(const llmlb_engine* e, llmlb_health* out);
+
+typedef struct llmlb_prefix_cache_stats {   /* llmlb_engine_config.prefix_cache; all 0 with the cache off */
+  uint32_t cached_pages;           /* pages in the cache, held by requests or evictable */
+  uint32_t evictable_pages;        /* cached pages no request holds */
+  uint64_t lookups;                /* admissions that walked the cache */
+  uint64_t hit_tokens;             /* context tokens those admissions did not prefill (64 per matched page) */
+  uint64_t published_pages;        /* pages entered into the cache */
+  uint64_t evicted_pages;          /* cached pages taken back for new KV */
+} llmlb_prefix_cache_stats;
+int llmlb_engine_prefix_cache_stats(const llmlb_engine* e, llmlb_prefix_cache_stats* out);
 
 /* --------------------------------------------------------------- requests --- */
 
@@ -238,6 +270,10 @@ int llmlb_request_submit_prompt_logprobs(llmlb_engine* e, const int32_t* prompt_
  * submitted otherwise delivers none; an unknown id returns LLMLB_E_NOT_FOUND. */
 int llmlb_request_poll_prompt_logprobs(llmlb_engine* e, uint64_t req_id, llmlb_token_logprobs* out, uint32_t cap,
                                        uint32_t* n_out);
+/* OpenAI's usage.prompt_tokens_details.cached_tokens: the client prompt's tokens served from the prefix cache at the
+ * request's first admission, min(64 * matched pages, n_prompt).  0 before admission and with the cache off; an unknown
+ * id returns LLMLB_E_NOT_FOUND. */
+int llmlb_request_cached_tokens(llmlb_engine* e, uint64_t req_id, uint32_t* n);
 /* Drain up to cap events. timeout_ms: 0 = return at once, <0 = wait until at least one. */
 int llmlb_request_poll(llmlb_engine* e, uint64_t req_id, llmlb_token_event* out, uint32_t cap,
                        uint32_t* n_out, int timeout_ms);

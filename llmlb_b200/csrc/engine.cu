@@ -12,6 +12,7 @@
 #include <cuda.h>
 
 #include <algorithm>
+#include <array>
 #include <chrono>
 #include <cmath>
 #include <condition_variable>
@@ -22,7 +23,9 @@
 #include <map>
 #include <memory>
 #include <mutex>
+#include <set>
 #include <thread>
+#include <tuple>
 #include <unordered_map>
 #include <vector>
 
@@ -208,6 +211,10 @@ struct Request {
   std::vector<int32_t> gen; // harvested generated tokens
   uint32_t gen_in_prompt = 0;
   uint32_t pages_published = 0;   // entries of `pages` already in the device block table
+  // prefix cache: the cached pages this request holds a reference on, for context pages 0, 1, ... in order.  chain[j] is
+  // pages[j], except where another request had cached the same key first: then pages[j] stays private (freed at release)
+  std::vector<int32_t> chain;
+  uint32_t cached_tokens = 0;     // client prompt tokens served from the cache at the first admission
   uint32_t preempted = 0;
   bool admitted_once = false;
   bool finished = false;
@@ -350,6 +357,88 @@ struct PlanChannel {
   }
 };
 
+// ---- prefix cache (llmlb_engine_config.prefix_cache) -------------------------------------------------------------------
+// Full KV pages by content: a tree whose node key is (parent page, the page's 64 token ids), compared exactly.  Every
+// decision iterates ordered containers only, so follower ranks replaying the plan channel reach the same state.  Host memory
+// is bounded by the pool: at most one key (64 ids) per page.  All members are under the engine's mu.
+struct PrefixCache {
+  struct Key {
+    int32_t parent;   // -1: positions 0..63
+    std::array<int32_t, kPageTokens> ids;
+    bool operator<(const Key& o) const { return parent != o.parent ? parent < o.parent : ids < o.ids; }
+  };
+  using Index = std::map<Key, int32_t>;
+  struct Node {
+    Index::iterator key;
+    bool cached = false;
+    uint32_t refs = 0;       // requests holding the page; 0 = evictable
+    uint32_t depth = 0;      // page index within its context
+    uint32_t children = 0;   // cached pages whose parent this is
+    uint64_t stamp = 0;      // release tick at which refs last reached 0
+  };
+  Index index;
+  std::vector<Node> node;                                    // by physical page
+  std::set<std::tuple<uint64_t, int64_t, int32_t>> lru;      // evictable pages: (stamp, -depth, page), first = next victim
+  uint64_t tick = 0;
+  uint64_t lookups = 0, hit_tokens = 0, published = 0, evicted = 0;
+
+  bool on() const { return !node.empty(); }
+  bool shared(int32_t page) const { return on() && node[page].cached; }
+  int32_t find(int32_t parent, const int32_t* ids) const {
+    Key k{parent, {}};
+    std::copy(ids, ids + kPageTokens, k.ids.begin());
+    auto it = index.find(k);
+    return it == index.end() ? -1 : it->second;
+  }
+  void ref(int32_t p) {
+    Node& n = node[p];
+    if (n.refs++ == 0) lru.erase(std::make_tuple(n.stamp, -int64_t(n.depth), p));
+  }
+  void unref(int32_t p) {   // callers advance `tick` once per release, so a request's pages share one stamp
+    Node& n = node[p];
+    if (--n.refs == 0) { n.stamp = tick; lru.insert(std::make_tuple(n.stamp, -int64_t(n.depth), p)); }
+  }
+  // page p (private, full, its KV launched) under `parent` with these ids; returns the cached page now holding the key,
+  // referenced once more: p itself, or the page cached before it
+  int32_t publish(int32_t parent, const int32_t* ids, uint32_t depth, int32_t p) {
+    Key k{parent, {}};
+    std::copy(ids, ids + kPageTokens, k.ids.begin());
+    auto ins = index.emplace(k, p);
+    const int32_t q = ins.first->second;
+    if (!ins.second) { ref(q); return q; }
+    Node& n = node[p];
+    n = Node{};
+    n.key = ins.first; n.cached = true; n.refs = 1; n.depth = depth;
+    if (parent >= 0) node[parent].children++;
+    published++;
+    return p;
+  }
+  // the least recently released evictable page, out of the cache (a leaf: its children were released no later, and are
+  // deeper); -1 if none
+  int32_t evict() {
+    if (lru.empty()) return -1;
+    const int32_t p = std::get<2>(*lru.begin());
+    lru.erase(lru.begin());
+    drop(p);
+    evicted++;
+    return p;
+  }
+  // every page back to `free` (none may be held), in page order
+  void clear(std::vector<int32_t>* free) {
+    for (int32_t p = 0; p < int32_t(node.size()); ++p)
+      if (node[p].cached) free->push_back(p);
+    index.clear();
+    lru.clear();
+    std::fill(node.begin(), node.end(), Node{});
+  }
+  void drop(int32_t p) {
+    Node& n = node[p];
+    if (n.key->first.parent >= 0) node[n.key->first.parent].children--;
+    index.erase(n.key);
+    n = Node{};
+  }
+};
+
 struct LayerW {
   __nv_bfloat16 *wqkv, *wo, *wgu, *wdown, *attn_norm, *ffn_norm;
   CUtensorMap m_wqkv, m_wo, m_wgu, m_wdown;
@@ -384,6 +473,7 @@ struct llmlb_engine {
   float* rope = nullptr;
   int32_t* d_block_tables = nullptr;  // [max_seqs][pages_per_seq]
   std::vector<int32_t> free_pages;
+  PrefixCache pc;                     // node table sized n_pages when cfg.prefix_cache is set, empty otherwise
   std::vector<int32_t> free_slots;
 
   // activations
@@ -531,7 +621,34 @@ struct llmlb_engine {
   // would dangle, and for a request the client already released the container holds the LAST owner (found by ASan over the
   // fake CUDA runtime: heap-use-after-free in finish_request on cancel of a released, running request)
   void finish_request(ReqPtr r, uint32_t reason);
-  void release_resources(ReqPtr r);
+  void release_resources(ReqPtr r, bool publish = true);
+  // a page for new KV: the free pool first, then the least recently released evictable cached page (mu held)
+  bool take_page(int32_t* p) {
+    if (!free_pages.empty()) { *p = free_pages.back(); free_pages.pop_back(); return true; }
+    return (*p = pc.evict()) >= 0;
+  }
+  size_t pages_available() const { return free_pages.size() + pc.lru.size(); }
+  // the cached chain along r's context: at most (n - 1) / 64 pages, so at least one token is prefilled (mu held)
+  void pc_match(const Request& r, std::vector<int32_t>* out) const {
+    out->clear();
+    const uint32_t max_match = (uint32_t(r.prompt.size()) - 1) / kPageTokens;
+    for (int32_t parent = -1; out->size() < max_match; ) {
+      parent = pc.find(parent, r.prompt.data() + out->size() * kPageTokens);
+      if (parent < 0) break;
+      out->push_back(parent);
+    }
+  }
+  // cache r's full pages whose positions are all below `limit` (mu held)
+  void pc_publish(Request& r, uint32_t limit) {
+    for (uint32_t j = uint32_t(r.chain.size()); (j + 1) * kPageTokens <= limit && j < r.pages.size(); ++j) {
+      int32_t ids[kPageTokens];
+      for (uint32_t i = 0; i < uint32_t(kPageTokens); ++i) {
+        const uint32_t pos = j * kPageTokens + i;
+        ids[i] = pos < r.prompt.size() ? r.prompt[pos] : r.gen[pos - r.n_prompt0];
+      }
+      r.chain.push_back(pc.publish(j ? r.chain[j - 1] : -1, ids, j, r.pages[j]));
+    }
+  }
   void preempt(ReqPtr r);
   void expire_requests();     // leader / single rank: queue timeouts and request deadlines (time-based)
   std::atomic<uint64_t> preemptions{0};
@@ -612,6 +729,7 @@ int llmlb_engine::init() {
   LLMLB_CUDA_CHECK(cudaStreamSynchronize(st));
   if (tp == 1) RC(warmup());
   for (int32_t p = int32_t(n_pages) - 1; p >= 0; --p) free_pages.push_back(p);
+  if (cfg.prefix_cache) pc.node.resize(n_pages);
   for (int32_t s = int32_t(cfg.max_seqs) - 1; s >= 0; --s) free_slots.push_back(s);
   worker = std::thread([this] { this->loop(); });
   return LLMLB_OK;
@@ -1166,7 +1284,7 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
   bool lp_rows = false;    // some finished row reports logprobs
   for (size_t i = 0; i < reqs.size(); ++i) {
     Request& r = *reqs[i];
-    if (r.prefilled == 0) {  // first chunk: publish block table + sampler state
+    if (r.pages_published == 0) {  // first chunk of this admission: publish block table + sampler state
       LLMLB_CUDA_CHECK(cudaMemcpyAsync(d_block_tables + size_t(r.slot) * pages_per_seq, r.pages.data(),
                                        r.pages.size() * 4, cudaMemcpyHostToDevice, st));
       slot_init_kernel<<<1, 1, 0, st>>>(S, r.slot, r.s.temperature, r.s.top_p, (int32_t)r.s.top_k, r.s.seed, uint64_t(r.harvested),
@@ -1185,6 +1303,8 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
       r.pages_published = uint32_t(r.pages.size());
     }
     const uint32_t p0 = r.prefilled;
+    for (uint32_t pg = p0 / kPageTokens; pc.on() && pg <= (p0 + take[i] - 1) / kPageTokens; ++pg)
+      if (pc.shared(r.pages[pg])) { set_error("prefix cache: a prefill step would write into a cached page"); return LLMLB_E_INTERNAL; }
     for (uint32_t j = 0; j < take[i]; ++j) {
       uint32_t pos = p0 + j;
       s_ids[row + j] = r.prompt[pos];
@@ -1270,6 +1390,7 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
     for (size_t i = 0; i < reqs.size(); ++i) {
       reqs[i]->prefilled += take[i];
       if (reqs[i]->prefilled == reqs[i]->prompt.size()) reqs[i]->launched = reqs[i]->harvested + 1;
+      if (pc.on()) pc_publish(*reqs[i], reqs[i]->prefilled);   // later steps that read them are ordered after this one
     }
     steps_prefill++;
     tokens_prefill += T;
@@ -1305,6 +1426,11 @@ int llmlb_engine::run_decode(const std::vector<ReqPtr>& batch) {
       }
     }
   }
+  for (auto& r : batch)   // the page that receives the input token's KV
+    if (pc.shared(r->pages[(r->n_prompt0 + r->launched - 1) / kPageTokens])) {
+      set_error("prefix cache: a decode step would write into a cached page");
+      return LLMLB_E_INTERNAL;
+    }
   InflightStep step;
   step.n_tokens = nb;
   step.reqs = batch;
@@ -1326,12 +1452,24 @@ int llmlb_engine::run_decode(const std::vector<ReqPtr>& batch) {
   return LLMLB_OK;
 }
 
-void llmlb_engine::release_resources(ReqPtr r) {  // mu held
+// publish: cache the full pages whose every position was the input of a launched step (prefilled context, and generated
+// tokens that a harvested token followed: in-flight steps only write positions beyond those).  Duplicates and private
+// pages go back to the free pool, cached ones are released.
+void llmlb_engine::release_resources(ReqPtr r, bool publish) {  // mu held
   if (r->slot >= 0) {
     free_slots.push_back(r->slot);
     r->slot = -1;
   }
-  for (int32_t p : r->pages) free_pages.push_back(p);
+  if (pc.on() && !r->pages.empty()) {
+    uint32_t limit = r->prefilled;
+    if (r->prefilled == r->prompt.size() && r->harvested > 0) limit = std::max(limit, r->n_prompt0 + r->harvested - 1);
+    if (publish) pc_publish(*r, limit);
+    pc.tick++;
+    for (int32_t p : r->chain) pc.unref(p);
+  }
+  for (size_t j = 0; j < r->pages.size(); ++j)
+    if (j >= r->chain.size() || r->chain[j] != r->pages[j]) free_pages.push_back(r->pages[j]);
+  r->chain.clear();
   r->pages.clear();
   r->pages_published = 0;
   running.erase(std::remove(running.begin(), running.end(), r), running.end());
@@ -1341,12 +1479,12 @@ void llmlb_engine::release_resources(ReqPtr r) {  // mu held
 // queue with its context extended by what it generated (recomputed at re-admission).  Only called
 // with nothing in flight, so every launched token has been harvested.  mu held.
 void llmlb_engine::preempt(ReqPtr r) {
+  release_resources(r);   // first: it publishes from the context as it was computed
   r->prompt.insert(r->prompt.end(), r->gen.begin() + r->gen_in_prompt, r->gen.end());
   r->gen_in_prompt = uint32_t(r->gen.size());
   r->prefilled = 0;
   r->launched = r->harvested;
   r->preempted++;
-  release_resources(r);
   waiting.push_front(r);
   preemptions++;
 }
@@ -1377,7 +1515,7 @@ void llmlb_engine::finish_request(ReqPtr r, uint32_t reason) {  // mu held
       if (r->top_logprobs >= 0) r->lp_events.push_back(no_logprobs());
     }
   }
-  release_resources(r);
+  release_resources(r, reason != LLMLB_FINISH_ERROR);   // the KV of a failed step is not trusted
   if (r->client_released) requests.erase(r->id);
   cv_events.notify_all();
 }
@@ -1464,19 +1602,34 @@ bool llmlb_engine::sched_iteration(std::unique_lock<std::mutex>& lk) {
     // sequence had generated) and token budget exist.  Pages for generated tokens are taken one at a
     // time as a sequence crosses a page boundary; when the pool runs dry the most recently admitted
     // sequence is evicted and recomputed later (below).
+    // With the prefix cache the context's cached chain comes first and needs no new page; evictable pages count as free.
+    std::vector<int32_t> hit;
     while (!waiting.empty() && budget > 0 && !free_slots.empty()) {
       ReqPtr r = waiting.front();
-      uint32_t need = ceil_div((uint32_t)r->prompt.size(), kPageTokens);
+      hit.clear();
+      if (pc.on() && !r->prompt_lp) pc_match(*r, &hit);   // prompt records need every prompt row's logits
+      uint32_t need = ceil_div((uint32_t)r->prompt.size(), kPageTokens) - uint32_t(hit.size());
+      size_t avail = pages_available();
+      for (int32_t p : hit) avail -= pc.node[p].refs == 0;   // a matched evictable page stops being evictable
       // first admission keeps one page per running sequence in reserve, so that admitting does not
       // immediately force an eviction
       const size_t reserve = r->admitted_once ? 0 : running.size();
-      if (need + reserve > free_pages.size() && !(running.empty() && need <= free_pages.size())) break;
+      if (need + reserve > avail && !(running.empty() && need <= avail)) break;
       waiting.pop_front();
       r->slot = free_slots.back(); free_slots.pop_back();
-      for (uint32_t i = 0; i < need; ++i) { r->pages.push_back(free_pages.back()); free_pages.pop_back(); }
+      if (pc.on() && !r->prompt_lp) {
+        pc.lookups++;
+        pc.hit_tokens += uint64_t(hit.size()) * kPageTokens;
+        for (int32_t p : hit) pc.ref(p);
+        r->pages = hit;
+        r->chain = hit;
+        r->prefilled = uint32_t(hit.size()) * kPageTokens;
+        if (!r->admitted_once) r->cached_tokens = std::min(r->prefilled, r->n_prompt0);
+      }
+      for (uint32_t i = 0; i < need; ++i) { int32_t p; take_page(&p); r->pages.push_back(p); }
       r->admitted_once = true;
       running.push_back(r);
-      uint32_t t = std::min<uint32_t>(budget, (uint32_t)r->prompt.size());
+      uint32_t t = std::min<uint32_t>(budget, (uint32_t)r->prompt.size() - r->prefilled);
       pf_reqs.push_back(r); pf_take.push_back(t); budget -= t;
     }
     if (pf_reqs.empty()) {
@@ -1488,8 +1641,9 @@ bool llmlb_engine::sched_iteration(std::unique_lock<std::mutex>& lk) {
       for (auto& r : dec) {
         const uint32_t need = ceil_div(r->n_prompt0 + r->launched, kPageTokens);
         while (r->pages.size() < need) {
-          if (free_pages.empty()) { shortage = true; break; }
-          r->pages.push_back(free_pages.back()); free_pages.pop_back();
+          int32_t p;
+          if (!take_page(&p)) { shortage = true; break; }
+          r->pages.push_back(p);
         }
         if (shortage) break;
       }
@@ -1742,13 +1896,36 @@ extern "C" int llmlb_engine_health(const llmlb_engine* ce, llmlb_health* out) {
   std::lock_guard<std::mutex> lk(e->mu);
   out->active_requests = (uint32_t)e->running.size();
   out->queued_requests = (uint32_t)e->waiting.size();
-  out->free_kv_pages = (uint32_t)e->free_pages.size();
+  out->free_kv_pages = (uint32_t)e->pages_available();   // evictable cached pages are free for any new KV
   out->total_kv_pages = e->n_pages;
   out->steps_prefill = e->steps_prefill; out->steps_decode = e->steps_decode;
   out->tokens_prefill = e->tokens_prefill; out->tokens_decode = e->tokens_decode;
   out->gpu_ms_prefill = e->gpu_ms_prefill; out->gpu_ms_decode = e->gpu_ms_decode;
   out->kernel_launches = g_kernel_launches.load();
   out->preemptions = e->preemptions.load();
+  return LLMLB_OK;
+}
+
+extern "C" int llmlb_engine_prefix_cache_stats(const llmlb_engine* ce, llmlb_prefix_cache_stats* out) {
+  llmlb_engine* e = const_cast<llmlb_engine*>(ce);
+  if (!e || !out) { set_error("llmlb_engine_prefix_cache_stats: null argument"); return LLMLB_E_INVALID_ARG; }
+  memset(out, 0, sizeof(*out));
+  std::lock_guard<std::mutex> lk(e->mu);
+  out->cached_pages = uint32_t(e->pc.index.size());
+  out->evictable_pages = uint32_t(e->pc.lru.size());
+  out->lookups = e->pc.lookups;
+  out->hit_tokens = e->pc.hit_tokens;
+  out->published_pages = e->pc.published;
+  out->evicted_pages = e->pc.evicted;
+  return LLMLB_OK;
+}
+
+extern "C" int llmlb_request_cached_tokens(llmlb_engine* e, uint64_t req_id, uint32_t* n) {
+  if (!e || !n) { set_error("llmlb_request_cached_tokens: null argument"); return LLMLB_E_INVALID_ARG; }
+  std::lock_guard<std::mutex> lk(e->mu);
+  auto it = e->requests.find(req_id);
+  if (it == e->requests.end()) { set_error("unknown request id"); return LLMLB_E_NOT_FOUND; }
+  *n = it->second->cached_tokens;
   return LLMLB_OK;
 }
 
@@ -2114,6 +2291,14 @@ extern "C" int llmlb_engine_load_tensor(llmlb_engine* e, const char* name, const
   }
   cudaSetDevice(e->cfg.device);
   std::lock_guard<std::mutex> sl(e->step_mu);
+  {
+    std::lock_guard<std::mutex> lk(e->mu);
+    // cached KV would be stale, and tensor-parallel ranks flushing at different points would split their plans
+    if (e->pc.on() && e->served) {
+      set_error("llmlb_engine_load_tensor: with prefix_cache, only before the first request or debug call");
+      return LLMLB_E_UNSUPPORTED;
+    }
+  }
   LLMLB_CUDA_CHECK(cudaStreamSynchronize(e->st));
   const __nv_bfloat16* src = (const __nv_bfloat16*)host + r0 * fc + c0;
   LLMLB_CUDA_CHECK(cudaMemcpy2D(base, ld * 2, src, fc * 2, c * 2, r, cudaMemcpyHostToDevice));
@@ -2165,6 +2350,8 @@ static int debug_acquire(llmlb_engine* e) {  // step_mu held
   }
   e->served = true;
   if (e->debug_slot < 0) {
+    // drop the prefix cache: an idle engine holds no cached page, and the hooks' prefill overwrites its pages
+    e->pc.clear(&e->free_pages);
     if (e->free_slots.empty() || e->free_pages.size() < e->pages_per_seq) { set_error("no free slot/pages"); return LLMLB_E_QUEUE_FULL; }
     e->debug_slot = e->free_slots.back(); e->free_slots.pop_back();
     for (uint32_t i = 0; i < e->pages_per_seq; ++i) { e->debug_pages.push_back(e->free_pages.back()); e->free_pages.pop_back(); }

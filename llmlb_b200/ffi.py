@@ -31,7 +31,7 @@ class EngineConfig(C.Structure):
                 ("synthetic_seed", C.c_uint64), ("use_cuda_graphs", C.c_uint32),
                 ("gemm_impl", C.c_uint32), ("lookahead", C.c_uint32), ("queue_max", C.c_uint32),
                 ("queue_timeout_ms", C.c_uint32), ("request_timeout_ms", C.c_uint32), ("attn_impl", C.c_uint32),
-                ("tp_proto", C.c_uint32), ("reserved", C.c_uint32 * 3)]
+                ("tp_proto", C.c_uint32), ("prefix_cache", C.c_uint32), ("reserved", C.c_uint32 * 2)]
 
 
 class ModelInfo(C.Structure):
@@ -47,6 +47,11 @@ class Health(C.Structure):
                 ("steps_decode", C.c_uint64), ("tokens_prefill", C.c_uint64),
                 ("tokens_decode", C.c_uint64), ("gpu_ms_prefill", C.c_double),
                 ("gpu_ms_decode", C.c_double), ("kernel_launches", C.c_uint64), ("preemptions", C.c_uint64)]
+
+
+class PrefixCacheStats(C.Structure):
+    _fields_ = [("cached_pages", C.c_uint32), ("evictable_pages", C.c_uint32), ("lookups", C.c_uint64),
+                ("hit_tokens", C.c_uint64), ("published_pages", C.c_uint64), ("evicted_pages", C.c_uint64)]
 
 
 class Sampling(C.Structure):
@@ -89,6 +94,7 @@ PROTOTYPES = {
     "llmlb_engine_set_rope_freq_factors": (C.c_int, [vp, _P(f32), u32]),
     "llmlb_engine_model_info": (C.c_int, [vp, _P(ModelInfo)]),
     "llmlb_engine_health": (C.c_int, [vp, _P(Health)]),
+    "llmlb_engine_prefix_cache_stats": (C.c_int, [vp, _P(PrefixCacheStats)]),
     "llmlb_engine_pause": (C.c_int, [vp, u32]),
     "llmlb_request_submit": (C.c_int, [vp, _P(i32), u32, _P(Sampling), _P(u64)]),
     "llmlb_request_submit_penalized": (C.c_int, [vp, _P(i32), u32, _P(Sampling), _P(Penalties), _P(u64)]),
@@ -97,6 +103,7 @@ PROTOTYPES = {
     "llmlb_request_poll_logprobs": (C.c_int, [vp, u64, _P(TokenEvent), _P(TokenLogprobs), u32, _P(u32), C.c_int]),
     "llmlb_request_submit_prompt_logprobs": (C.c_int, [vp, _P(i32), u32, _P(Sampling), _P(Penalties), u32, _P(u64)]),
     "llmlb_request_poll_prompt_logprobs": (C.c_int, [vp, u64, _P(TokenLogprobs), u32, _P(u32)]),
+    "llmlb_request_cached_tokens": (C.c_int, [vp, u64, _P(u32)]),
     "llmlb_request_cancel": (C.c_int, [vp, u64]),
     "llmlb_request_release": (C.c_int, [vp, u64]),
     "llmlb_debug_prefill_logits": (C.c_int, [vp, _P(i32), u32, _P(f32), _P(f32)]),
@@ -182,7 +189,7 @@ class Engine:
     def __init__(self, model, model_id="llama-3-8b-synthetic", device=0, tp_rank=0, tp_size=1,
                  max_seqs=8, max_ctx=1024, kv_pages=0, max_step_tokens=0, seed=0,
                  use_cuda_graphs=True, gemm_impl=0, lookahead=0, queue_max=0, queue_timeout_ms=0, request_timeout_ms=0, attn_impl=0, tp_proto=0,
-                 rope_freq_factors=None):
+                 rope_freq_factors=None, prefix_cache=False):
         cfg = EngineConfig()
         cfg.abi_version = ABI_VERSION
         for k, v in model.items():
@@ -196,6 +203,7 @@ class Engine:
         cfg.gemm_impl, cfg.lookahead = gemm_impl, lookahead
         cfg.queue_max, cfg.queue_timeout_ms, cfg.request_timeout_ms = queue_max, queue_timeout_ms, request_timeout_ms
         cfg.attn_impl, cfg.tp_proto = attn_impl, tp_proto
+        cfg.prefix_cache = 1 if prefix_cache else 0
         self.model = dict(model)
         self.cfg = cfg
         self._h = vp()
@@ -303,6 +311,12 @@ class Engine:
         check(lib().llmlb_request_poll_prompt_logprobs(self._h, rid, lp, cap, C.byref(n)))
         return [dict(logprob=r.logprob, top_logprobs=[(r.top_ids[i], r.top_logprobs[i]) for i in range(r.n_top)]) for r in lp[:n.value]]
 
+    def cached_tokens(self, rid):
+        """The prompt tokens served from the prefix cache at the request's first admission (0 before it)."""
+        n = u32()
+        check(lib().llmlb_request_cached_tokens(self._h, rid, C.byref(n)))
+        return n.value
+
     def generate(self, prompt_ids, max_tokens, **kw):
         """submit + drain; returns (token ids, events).  With logprobs=, the events carry them (poll_logprobs)."""
         rid = self.submit(prompt_ids, max_tokens, **kw)
@@ -332,6 +346,11 @@ class Engine:
         h = Health()
         check(lib().llmlb_engine_health(self._h, C.byref(h)))
         return {k: getattr(h, k) for k, _ in Health._fields_}
+
+    def prefix_cache_stats(self):
+        st = PrefixCacheStats()
+        check(lib().llmlb_engine_prefix_cache_stats(self._h, C.byref(st)))
+        return {k: getattr(st, k) for k, _ in PrefixCacheStats._fields_}
 
     def model_info(self):
         m = ModelInfo()

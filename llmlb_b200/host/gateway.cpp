@@ -532,19 +532,26 @@ Json chat_chunk(const std::string& id, const std::string& model, int64_t created
   root.set("choices", choices);
   return root;
 }
-static Json chat_usage(uint32_t p, uint32_t c) {
+static Json cached_details(uint32_t n) {
+  Json d = Json::object();
+  d.set("cached_tokens", n);
+  return d;
+}
+static Json chat_usage(uint32_t p, uint32_t c, const uint32_t* cached) {
   Json u = Json::object();
   u.set("prompt_tokens", p); u.set("completion_tokens", c); u.set("total_tokens", p + c);
+  if (cached) u.set("prompt_tokens_details", cached_details(*cached));
   return u;
 }
-Json chat_usage_chunk(const std::string& id, const std::string& model, int64_t created, uint32_t p, uint32_t c) {
+Json chat_usage_chunk(const std::string& id, const std::string& model, int64_t created, uint32_t p, uint32_t c, const uint32_t* cached) {
   Json root = Json::object();
   root.set("id", id); root.set("object", "chat.completion.chunk"); root.set("created", created);
-  root.set("model", model); root.set("choices", Json::array()); root.set("usage", chat_usage(p, c));
+  root.set("model", model); root.set("choices", Json::array()); root.set("usage", chat_usage(p, c, cached));
   return root;
 }
 Json chat_completion_body(const std::string& id, const std::string& model, int64_t created,
-                          const std::string& content, const char* finish_reason, uint32_t p, uint32_t c, const Json* logprobs) {
+                          const std::string& content, const char* finish_reason, uint32_t p, uint32_t c, const Json* logprobs,
+                          const uint32_t* cached) {
   Json msg = Json::object(); msg.set("role", "assistant"); msg.set("content", content);
   Json choice = Json::object();
   choice.set("index", 0); choice.set("message", msg);
@@ -553,11 +560,12 @@ Json chat_completion_body(const std::string& id, const std::string& model, int64
   Json choices = Json::array(); choices.push(choice);
   Json root = Json::object();
   root.set("id", id); root.set("object", "chat.completion"); root.set("created", created); root.set("model", model);
-  root.set("choices", choices); root.set("usage", chat_usage(p, c));
+  root.set("choices", choices); root.set("usage", chat_usage(p, c, cached));
   return root;
 }
 Json completion_body(const std::string& id, const std::string& model, int64_t created,
-                     const std::string& text, const char* finish_reason, uint32_t p, uint32_t c, const Json* logprobs) {
+                     const std::string& text, const char* finish_reason, uint32_t p, uint32_t c, const Json* logprobs,
+                     const uint32_t* cached) {
   Json choice = Json::object();
   choice.set("index", 0); choice.set("text", text);
   if (logprobs) choice.set("logprobs", *logprobs);
@@ -565,7 +573,7 @@ Json completion_body(const std::string& id, const std::string& model, int64_t cr
   Json choices = Json::array(); choices.push(choice);
   Json root = Json::object();
   root.set("id", id); root.set("object", "text_completion"); root.set("created", created); root.set("model", model);
-  root.set("choices", choices); root.set("usage", chat_usage(p, c));
+  root.set("choices", choices); root.set("usage", chat_usage(p, c, cached));
   return root;
 }
 Json completion_chunk(const std::string& id, const std::string& model, int64_t created, const std::string* text, const char* finish_reason,
@@ -579,10 +587,11 @@ Json completion_chunk(const std::string& id, const std::string& model, int64_t c
   root.set("choices", choices);
   return root;
 }
-Json completion_usage_chunk(const std::string& id, const std::string& model, int64_t created, uint32_t p, uint32_t c) {
+Json completion_usage_chunk(const std::string& id, const std::string& model, int64_t created, uint32_t p, uint32_t c,
+                            const uint32_t* cached) {
   Json root = Json::object();
   root.set("id", id); root.set("object", "text_completion"); root.set("created", created);
-  root.set("model", model); root.set("choices", Json::array()); root.set("usage", chat_usage(p, c));
+  root.set("model", model); root.set("choices", Json::array()); root.set("usage", chat_usage(p, c, cached));
   return root;
 }
 // OpenAI writes a log-probability it cannot represent (-inf) as -9999.0
@@ -630,20 +639,21 @@ Json completion_logprobs(const std::vector<LogprobEntry>& entries) {
   return root;
 }
 
-static Json resp_usage(uint32_t i, uint32_t o) {
+static Json resp_usage(uint32_t i, uint32_t o, const uint32_t* cached) {
   Json u = Json::object();
   u.set("input_tokens", i); u.set("output_tokens", o); u.set("total_tokens", i + o);
+  if (cached) u.set("input_tokens_details", cached_details(*cached));
   return u;
 }
 Json responses_body(const std::string& id, const std::string& model, int64_t created,
-                    const std::string& text, uint32_t in, uint32_t out, const char* status) {
+                    const std::string& text, uint32_t in, uint32_t out, const char* status, const uint32_t* cached) {
   Json part = Json::object(); part.set("type", "output_text"); part.set("text", text);
   Json content = Json::array(); content.push(part);
   Json item = Json::object(); item.set("type", "message"); item.set("role", "assistant"); item.set("content", content);
   Json output = Json::array(); output.push(item);
   Json root = Json::object();
   root.set("id", id); root.set("object", "response"); root.set("created_at", created); root.set("model", model);
-  root.set("status", status); root.set("output", output); root.set("usage", resp_usage(in, out));
+  root.set("status", status); root.set("output", output); root.set("usage", resp_usage(in, out, cached));
   return root;
 }
 Json responses_event_created(const std::string& id, const std::string& model) {
@@ -669,9 +679,9 @@ Json responses_event_text_done(const std::string& t) {
   Json e = Json::object(); e.set("type", "response.output_text.done"); e.set("text", t);
   return e;
 }
-Json responses_event_done(const std::string& id, uint32_t in, uint32_t out) {
+Json responses_event_done(const std::string& id, uint32_t in, uint32_t out, const uint32_t* cached) {
   Json r = Json::object(); r.set("id", id); r.set("object", "response"); r.set("status", "completed");
-  r.set("usage", resp_usage(in, out));
+  r.set("usage", resp_usage(in, out, cached));
   Json e = Json::object(); e.set("type", "response.done"); e.set("response", r);
   return e;
 }

@@ -257,22 +257,25 @@ class StopMatcher {
 std::string sse_event(const Json& j);                       // "data: {...}\n\n"
 inline std::string sse_done() { return "data: [DONE]\n\n"; }
 // logprobs (optional): the choice's "logprobs" value (chat_logprobs / completion_logprobs); without it the shapes are the
-// ones above, byte for byte
+// ones above, byte for byte.  cached_tokens (optional, a prefix-cache engine): usage gains
+// "prompt_tokens_details":{"cached_tokens":N} ("input_tokens_details" on responses); without it usage is unchanged
 Json chat_chunk(const std::string& id, const std::string& model, int64_t created,
                 const std::string* role, const std::string* content, const char* finish_reason,
                 const Json* logprobs = nullptr);
 Json chat_usage_chunk(const std::string& id, const std::string& model, int64_t created,
-                      uint32_t prompt_tokens, uint32_t completion_tokens);
+                      uint32_t prompt_tokens, uint32_t completion_tokens, const uint32_t* cached_tokens = nullptr);
 Json chat_completion_body(const std::string& id, const std::string& model, int64_t created,
                           const std::string& content, const char* finish_reason,
-                          uint32_t prompt_tokens, uint32_t completion_tokens, const Json* logprobs = nullptr);
+                          uint32_t prompt_tokens, uint32_t completion_tokens, const Json* logprobs = nullptr,
+                          const uint32_t* cached_tokens = nullptr);
 // legacy /v1/completions stream: {"object":"text_completion","choices":[{"index":0,"text":...,"finish_reason":...}]}
 Json completion_chunk(const std::string& id, const std::string& model, int64_t created, const std::string* text, const char* finish_reason,
                       const Json* logprobs = nullptr);
-Json completion_usage_chunk(const std::string& id, const std::string& model, int64_t created, uint32_t prompt_tokens, uint32_t completion_tokens);
+Json completion_usage_chunk(const std::string& id, const std::string& model, int64_t created, uint32_t prompt_tokens, uint32_t completion_tokens,
+                            const uint32_t* cached_tokens = nullptr);
 Json completion_body(const std::string& id, const std::string& model, int64_t created,
                      const std::string& text, const char* finish_reason, uint32_t prompt_tokens,
-                     uint32_t completion_tokens, const Json* logprobs = nullptr);
+                     uint32_t completion_tokens, const Json* logprobs = nullptr, const uint32_t* cached_tokens = nullptr);
 
 // ---- OpenAI logprobs ----
 // One listed token (or one of its alternatives): text through from_utf8_lossy, raw bytes, log-probability.
@@ -292,13 +295,13 @@ Json chat_logprobs(const std::vector<LogprobEntry>& entries);
 Json completion_logprobs(const std::vector<LogprobEntry>& entries);
 Json responses_body(const std::string& id, const std::string& model, int64_t created,
                     const std::string& text, uint32_t input_tokens, uint32_t output_tokens,
-                    const char* status);
+                    const char* status, const uint32_t* cached_tokens = nullptr);
 Json responses_event_created(const std::string& id, const std::string& model);
 Json responses_event_item_added();
 Json responses_event_part_added();
 Json responses_event_delta(const std::string& delta);
 Json responses_event_text_done(const std::string& text);
-Json responses_event_done(const std::string& id, uint32_t input_tokens, uint32_t output_tokens);
+Json responses_event_done(const std::string& id, uint32_t input_tokens, uint32_t output_tokens, const uint32_t* cached_tokens = nullptr);
 
 // Byte-level placeholder tokenizer (no tokenizer assets exist on the box): ids 0..255 are raw
 // bytes shifted by 3 reserved ids; anything else renders as "<|id|>".

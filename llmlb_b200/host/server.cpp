@@ -42,6 +42,7 @@
 #pragma weak llmlb_request_poll_logprobs
 #pragma weak llmlb_request_submit_prompt_logprobs
 #pragma weak llmlb_request_poll_prompt_logprobs
+#pragma weak llmlb_request_cached_tokens
 #include "anthropic.hpp"
 #include "checkpoint.hpp"
 #include "download.hpp"
@@ -54,6 +55,7 @@ struct Server {
   llmlb_engine* eng = nullptr;
   std::string model_id, api_key;
   uint32_t vocab = 0, max_ctx = 0;
+  bool prefix_cache = false;   // --prefix-cache: the engine reuses cached prompt prefixes, usage reports cached_tokens
   LoadManager lm;
   InferenceGate gate;
   std::atomic<uint64_t> seq{0};
@@ -583,6 +585,9 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
                                  : sse_event(chat_chunk(id, jm->str(), created, nullptr, &rest, nullptr)));
     }
   }
+  // OpenAI's usage.prompt_tokens_details.cached_tokens (input_tokens_details on responses); /v1/messages keeps its shapes
+  uint32_t cached = 0;
+  const uint32_t* cp = G.prefix_cache && !anthropic && llmlb_request_cached_tokens(G.eng, rid, &cached) == LLMLB_OK ? &cached : nullptr;
   llmlb_request_release(G.eng, rid);
   const uint64_t ms = uint64_t(std::chrono::duration_cast<std::chrono::milliseconds>(std::chrono::steady_clock::now() - t0).count());
   // streaming drop still counts as success when tokens flowed (openai.rs:2556-2648)
@@ -618,12 +623,12 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
     std::string tail;
     if (kind == 0) {
       tail += sse_event(chat_chunk(id, jm->str(), created, nullptr, nullptr, fr));
-      if (include_usage) tail += sse_event(chat_usage_chunk(id, jm->str(), created, prompt_tokens, completion_tokens));
+      if (include_usage) tail += sse_event(chat_usage_chunk(id, jm->str(), created, prompt_tokens, completion_tokens, cp));
     } else if (kind == 1) {
-      tail += sse_event(responses_event_text_done(text)) + sse_event(responses_event_done(id, prompt_tokens, completion_tokens));
+      tail += sse_event(responses_event_text_done(text)) + sse_event(responses_event_done(id, prompt_tokens, completion_tokens, cp));
     } else {   // legacy completions: text_completion chunks, a finish chunk, optional usage
       tail += sse_event(completion_chunk(id, jm->str(), created, nullptr, fr));
-      if (include_usage) tail += sse_event(completion_usage_chunk(id, jm->str(), created, prompt_tokens, completion_tokens));
+      if (include_usage) tail += sse_event(completion_usage_chunk(id, jm->str(), created, prompt_tokens, completion_tokens, cp));
     }
     tail += sse_done();
     if (anthropic) {  // usage always travels to the transformer (message_delta carries output_tokens)
@@ -641,9 +646,9 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
   } else {
     const Json lj = lp_on ? lp_json(lp_all) : Json();
     const Json* lpp = lp_on ? &lj : nullptr;
-    Json body = kind == 0 ? chat_completion_body(id, jm->str(), created, text, fr, prompt_tokens, completion_tokens, lpp)
-              : kind == 1 ? responses_body(id, jm->str(), created, text, prompt_tokens, completion_tokens, "completed")
-                          : completion_body(id, jm->str(), created, prompt_text + text, fr, prompt_tokens, completion_tokens, lpp);
+    Json body = kind == 0 ? chat_completion_body(id, jm->str(), created, text, fr, prompt_tokens, completion_tokens, lpp, cp)
+              : kind == 1 ? responses_body(id, jm->str(), created, text, prompt_tokens, completion_tokens, "completed", cp)
+                          : completion_body(id, jm->str(), created, prompt_text + text, fr, prompt_tokens, completion_tokens, lpp, cp);
     send_json(fd, 200, body.dump());
   }
 }
@@ -834,7 +839,17 @@ int main(int argc, char** argv) {
   uint32_t queue_max = 100, queue_timeout_ms = 60000, request_timeout_ms = 120000;
   bool dry_run = false;
   G.model_id = "llama-3-8b";
-  for (int i = 1; i < argc; ++i) if (std::string(argv[i]) == "--dry-run") { dry_run = true; for (int j = i; j + 1 < argc; ++j) argv[j] = argv[j + 1]; --argc; --i; }
+  for (int i = 1; i < argc; ++i) {   // the flags without a value
+    const std::string a = argv[i];
+    if (a != "--dry-run" && a != "--prefix-cache") continue;
+    (a == "--dry-run" ? dry_run : G.prefix_cache) = true;
+    for (int j = i; j + 1 < argc; ++j) argv[j] = argv[j + 1];
+    --argc; --i;
+  }
+  if (G.prefix_cache && !llmlb_request_cached_tokens) {
+    fprintf(stderr, "--prefix-cache: the engine library this server runs on has no prefix cache (llmlb_request_cached_tokens is missing)\n");
+    return 2;
+  }
   for (int i = 1; i + 1 < argc; i += 2) {
     std::string k = argv[i], v = argv[i + 1];
     if (k == "--port") port = atoi(v.c_str()); else if (k == "--model") geometry = v;
@@ -885,6 +900,7 @@ int main(int argc, char** argv) {
   strncpy(cfg.model_id, G.model_id.c_str(), sizeof cfg.model_id - 1);
   cfg.tp_size = 1; cfg.max_seqs = max_seqs; cfg.max_ctx = max_ctx; cfg.kv_block_tokens = 64; cfg.use_cuda_graphs = 1;
   cfg.queue_max = queue_max; cfg.queue_timeout_ms = queue_timeout_ms; cfg.request_timeout_ms = request_timeout_ms;
+  cfg.prefix_cache = G.prefix_cache ? 1 : 0;
   G.vocab = cfg.model.vocab; G.max_ctx = max_ctx; G.queue_timeout_ms = queue_timeout_ms; G.request_timeout_ms = request_timeout_ms;
   // tokenizer: --tokenizer file, else the one a .gguf carries
   std::string tok_json, tok_src = tokenizer_path;

@@ -89,7 +89,8 @@ def check():
     hdr = open(HDR).read()
     structs = rust_structs(text)
     problems = []
-    want = ["llmlb_model_config", "llmlb_engine_config", "llmlb_model_info", "llmlb_health", "llmlb_sampling", "llmlb_token_event"]
+    want = ["llmlb_model_config", "llmlb_engine_config", "llmlb_model_info", "llmlb_health", "llmlb_sampling", "llmlb_token_event",
+            "llmlb_prefix_cache_stats"]
     for w in want:
         if w not in structs:
             problems.append("struct %s missing from lib.rs" % w)
