@@ -187,6 +187,7 @@ extern "C" {
     pub fn llmlb_request_submit_prompt_logprobs(e: *mut llmlb_engine, prompt_ids: *const i32, n_prompt: u32, s: *const llmlb_sampling, pen: *const llmlb_penalties, top_logprobs: u32, req_id: *mut u64) -> c_int;
     pub fn llmlb_request_poll_prompt_logprobs(e: *mut llmlb_engine, req_id: u64, out: *mut llmlb_token_logprobs, cap: u32, n_out: *mut u32) -> c_int;
     pub fn llmlb_request_cached_tokens(e: *mut llmlb_engine, req_id: u64, n: *mut u32) -> c_int;
+    pub fn llmlb_request_submit_choices(e: *mut llmlb_engine, prompt_ids: *const i32, n_prompt: u32, s: *const llmlb_sampling, pen: *const llmlb_penalties, top_logprobs: i32, prompt_logprobs: u32, n: u32, req_ids: *mut u64) -> c_int;
     pub fn llmlb_request_cancel(e: *mut llmlb_engine, req_id: u64) -> c_int;
     pub fn llmlb_request_release(e: *mut llmlb_engine, req_id: u64) -> c_int;
 }
@@ -335,6 +336,41 @@ impl Engine {
         };
         check(unsafe { llmlb_request_submit_penalized(self.raw, prompt_ids.as_ptr(), prompt_ids.len() as u32, &raw_s, &pen, &mut id) })?;
         Ok(id)
+    }
+
+    /// OpenAI's `n`: `n` choices of one prompt, prefilled once; returns their ids, choice `i` sampling with `seed + i`.
+    /// `top_logprobs`: `None` = no logprobs, `Some(0..=20)` alternatives per token (read with `llmlb_request_poll_logprobs`);
+    /// `prompt_logprobs` (with `top_logprobs`): the prompt's records too, delivered to every choice.
+    pub fn submit_choices(&self, prompt_ids: &[i32], s: &Sampling, n: u32, top_logprobs: Option<u32>, prompt_logprobs: bool)
+        -> Result<Vec<u64>, EngineError> {
+        let raw_s = llmlb_sampling {
+            max_tokens: s.max_tokens,
+            temperature: s.temperature,
+            top_k: s.top_k,
+            top_p: s.top_p,
+            seed: s.seed,
+            stop_ids: if s.stop_ids.is_empty() { std::ptr::null() } else { s.stop_ids.as_ptr() },
+            n_stop_ids: s.stop_ids.len() as u32,
+            ignore_eos: s.ignore_eos as u32,
+        };
+        let ids: Vec<i32> = s.logit_bias.iter().map(|b| b.0).collect();
+        let vals: Vec<f32> = s.logit_bias.iter().map(|b| b.1).collect();
+        let pen = llmlb_penalties {
+            frequency_penalty: s.frequency_penalty,
+            presence_penalty: s.presence_penalty,
+            bias_ids: if ids.is_empty() { std::ptr::null() } else { ids.as_ptr() },
+            bias_values: if vals.is_empty() { std::ptr::null() } else { vals.as_ptr() },
+            n_bias: ids.len() as u32,
+        };
+        let neutral = s.frequency_penalty == 0.0 && s.presence_penalty == 0.0 && s.logit_bias.is_empty();
+        let mut out = vec![0u64; n.max(1) as usize];
+        check(unsafe {
+            llmlb_request_submit_choices(self.raw, prompt_ids.as_ptr(), prompt_ids.len() as u32, &raw_s,
+                                         if neutral { std::ptr::null() } else { &pen }, top_logprobs.map_or(-1, |t| t as i32),
+                                         prompt_logprobs as u32, n, out.as_mut_ptr())
+        })?;
+        out.truncate(n as usize);
+        Ok(out)
     }
 
     /// Drains up to `buf.len()` events; `timeout` zero returns at once.  `Ok(0)` on timeout.

@@ -274,6 +274,23 @@ int llmlb_request_poll_prompt_logprobs(llmlb_engine* e, uint64_t req_id, llmlb_t
  * request's first admission, min(64 * matched pages, n_prompt).  0 before admission and with the cache off; an unknown
  * id returns LLMLB_E_NOT_FOUND. */
 int llmlb_request_cached_tokens(llmlb_engine* e, uint64_t req_id, uint32_t* n);
+/* OpenAI's n: n choices of one prompt.  The prompt is prefilled once; the choices then share its full KV pages and each
+ * gets its own copy of the last, partial page (llmlb_op_kv_fork), and they decode as ordinary sequences.  req_ids[i] is
+ * choice i, an ordinary request id for poll, poll_logprobs, poll_prompt_logprobs, cancel, release and cached_tokens.
+ *  - pen: NULL = no penalties; top_logprobs: -1 = no logprobs, 0..20 alternatives; prompt_logprobs (needs
+ *    top_logprobs >= 0): the prompt records, computed once and delivered to every choice.
+ *  - Seeds: choice i samples from the stream of seed s->seed + i (u64, wrapping), so choice 0 draws exactly what the
+ *    matching single request draws.
+ *  - n must be in [1, max_seqs], else LLMLB_E_INVALID_ARG naming n.  n == 1 is the matching single-request submit.
+ *  - Admission is atomic and FIFO: n slots and ceil(L/64) - matched + (n-1) * [L mod 64 != 0] pages for a prompt of L
+ *    tokens, with one prefix-cache lookup (every choice reports its cached_tokens).  The group counts as n requests
+ *    toward queue_max, active_requests and queued_requests; timeouts apply per choice.
+ *  - Cancelling one choice never ends another.  A choice cancelled before the fork ends CANCELLED with no token.  After the
+ *    fork a preempted choice gives up its shares and is recomputed alone from its own context.
+ *  - A KV page is returned to the pool when the last sequence holding it releases it. */
+int llmlb_request_submit_choices(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt, const llmlb_sampling* s,
+                                 const llmlb_penalties* pen, int32_t top_logprobs, uint32_t prompt_logprobs, uint32_t n,
+                                 uint64_t* req_ids);
 /* Drain up to cap events. timeout_ms: 0 = return at once, <0 = wait until at least one. */
 int llmlb_request_poll(llmlb_engine* e, uint64_t req_id, llmlb_token_event* out, uint32_t cap,
                        uint32_t* n_out, int timeout_ms);
@@ -395,6 +412,13 @@ int llmlb_op_logprobs(const float* logits, uint32_t n_rows, uint32_t vocab, cons
                       const int32_t* top_n, llmlb_token_logprobs* out_records, void* stream);
 /* a2.13 all-reduce(sum) of fp32 [n] across tp ranks through peer-mapped buffers. */
 int llmlb_op_allreduce(llmlb_engine* e, float* buf_f32, uint64_t n, void* stream);
+/* Copy rows [0, rows) of KV page src_page to the n_dst pages dst_pages (device int32 [n_dst]), in K and V, for every
+ * layer and every KV head of the pools ([n_layers][n_pages][n_kv][64][128] bf16).  Rows rows..63 of the destinations and
+ * every other page are left untouched; a destination id outside [0, n_pages) is skipped.  One launch (the request fork of
+ * llmlb_request_submit_choices).  n_layers in [1, 65535], n_kv in [1, 256], src_page in [0, n_pages), n_dst in
+ * [1, 1024], rows in [1, 64]; otherwise LLMLB_E_INVALID_ARG. */
+int llmlb_op_kv_fork(void* k_pool, void* v_pool, uint32_t n_layers, uint32_t n_pages, uint32_t n_kv, int32_t src_page,
+                     const int32_t* dst_pages, uint32_t n_dst, uint32_t rows, void* stream);
 
 /* synthetic weights: fills a [rows, cols] bf16 slice whose global origin is (row0, col0) in a
  * tensor with `ld` columns; value depends only on (seed, tensor_id, global index). */

@@ -15,7 +15,7 @@ OBJ = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libllmlb_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 SOURCES = ["elementwise.cu", "gemv.cu", "gemv_ks.cu", "gemm_tc.cu", "gemm_tc2.cu", "attention.cu", "attention_tc.cu",
-           "sampling.cu", "penalty.cu", "logprob.cu", "tp_exchange.cu", "engine.cu"]
+           "sampling.cu", "penalty.cu", "logprob.cu", "tp_exchange.cu", "kv_fork.cu", "engine.cu"]
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 

@@ -88,6 +88,8 @@ int penalty_reset_launch(int32_t* counts, uint64_t count_stride, float* freq, fl
                          float f, float p, uint32_t nb, uint32_t vocab, const int32_t* gen, uint32_t n_gen, cudaStream_t st);
 int logprob_launch(const float* logits, uint32_t n_rows, uint32_t vocab, const int32_t* tokens, const int32_t* top_n,
                    const int32_t* row_slot, llmlb_token_logprobs* out, cudaStream_t st);
+int kv_fork_launch(__nv_bfloat16* k_pool, __nv_bfloat16* v_pool, uint32_t n_layers, uint32_t n_pages, uint32_t n_kv,
+                   int32_t src_page, const int32_t* dst_pages, uint32_t n_dst, uint32_t rows, cudaStream_t st);
 int rope_append_launch(void* qkv, const int32_t* positions, const int32_t* page_of_token, const float* rope_table,
                        void* k_pages, void* v_pages, uint32_t n_tokens, uint32_t n_heads, uint32_t n_kv, bool pdl,
                        cudaStream_t st);
@@ -215,6 +217,10 @@ struct Request {
   // pages[j], except where another request had cached the same key first: then pages[j] stays private (freed at release)
   std::vector<int32_t> chain;
   uint32_t cached_tokens = 0;     // client prompt tokens served from the cache at the first admission
+  // n choices of one prompt (llmlb_request_submit_choices), until the fork: the group's unfinished choices in choice order,
+  // shared by all of them.  The first prefills the prompt for the group; the others wait in `running` with a slot and their
+  // own tail page (L mod 64 != 0).  Null for a lone request, and for every choice once its group has forked.
+  std::shared_ptr<std::vector<std::weak_ptr<Request>>> group;
   uint32_t preempted = 0;
   bool admitted_once = false;
   bool finished = false;
@@ -228,6 +234,16 @@ struct Request {
   std::chrono::steady_clock::time_point t_submit;
 };
 using ReqPtr = std::shared_ptr<Request>;
+
+// the choices of r's group that have not finished, in choice order (r alone without a group)
+static std::vector<ReqPtr> group_members(const ReqPtr& r) {
+  if (!r->group) return {r};
+  std::vector<ReqPtr> out;
+  for (auto& w : *r->group) out.push_back(w.lock());
+  return out;
+}
+// a choice waiting for its group's prefill: it is neither prefilled nor decoded until the fork
+static bool awaits_fork(const Request& r) { return r.group && r.group->front().lock().get() != &r; }
 
 struct InflightStep {
   cudaEvent_t ev_start = nullptr, ev_end = nullptr;
@@ -256,7 +272,8 @@ struct PlanHeader {
   uint64_t ring_bytes;
 };
 enum PlanEvent : uint32_t { kPlanSubmit = 1, kPlanCancel = 2, kPlanRelease = 3, kPlanPause = 4, kPlanSched = 5, kPlanHarvest = 6, kPlanStop = 7,
-                            kPlanExpire = 8 /* id + finish reason: a time-based decision of rank 0's clock */ };
+                            kPlanExpire = 8 /* id + finish reason: a time-based decision of rank 0's clock */,
+                            kPlanSubmitChoices = 9 /* [u32 n][u32 0] + a kPlanSubmit record: n choices, ids id .. id + n - 1 */ };
 constexpr uint32_t kPlanMagic = 0x4C4C5031u;   // "LLP1"
 constexpr size_t kPlanHeaderBytes = 4096, kPlanRingBytes = size_t(8) << 20;
 constexpr long long kPlanStallMs = 30000;   // a follower that has not drained an 8 MiB ring for this long is gone
@@ -371,7 +388,7 @@ struct PrefixCache {
   struct Node {
     Index::iterator key;
     bool cached = false;
-    uint32_t refs = 0;       // requests holding the page; 0 = evictable
+    uint32_t refs = 0;       // sequences holding the page (cached or not); a cached page nobody holds is evictable
     uint32_t depth = 0;      // page index within its context
     uint32_t children = 0;   // cached pages whose parent this is
     uint64_t stamp = 0;      // release tick at which refs last reached 0
@@ -382,8 +399,10 @@ struct PrefixCache {
   uint64_t tick = 0;
   uint64_t lookups = 0, hit_tokens = 0, published = 0, evicted = 0;
 
-  bool on() const { return !node.empty(); }
-  bool shared(int32_t page) const { return on() && node[page].cached; }
+  bool enabled = false;                                      // llmlb_engine_config.prefix_cache
+  bool on() const { return enabled; }
+  // a page no step may write into: cached, or held by more than one sequence (the choices of a request share its prompt)
+  bool shared(int32_t page) const { return node[page].cached || node[page].refs > 1; }
   int32_t find(int32_t parent, const int32_t* ids) const {
     Key k{parent, {}};
     std::copy(ids, ids + kPageTokens, k.ids.begin());
@@ -392,23 +411,30 @@ struct PrefixCache {
   }
   void ref(int32_t p) {
     Node& n = node[p];
-    if (n.refs++ == 0) lru.erase(std::make_tuple(n.stamp, -int64_t(n.depth), p));
+    if (n.refs++ == 0 && n.cached) lru.erase(std::make_tuple(n.stamp, -int64_t(n.depth), p));
   }
-  void unref(int32_t p) {   // callers advance `tick` once per release, so a request's pages share one stamp
+  // true: nobody holds p any more and it is not cached, so it goes back to the free list.  Callers advance `tick` once per
+  // release, so a request's pages share one stamp
+  bool unref(int32_t p) {
     Node& n = node[p];
-    if (--n.refs == 0) { n.stamp = tick; lru.insert(std::make_tuple(n.stamp, -int64_t(n.depth), p)); }
+    if (--n.refs) return false;
+    if (!n.cached) return true;
+    n.stamp = tick;
+    lru.insert(std::make_tuple(n.stamp, -int64_t(n.depth), p));
+    return false;
   }
-  // page p (private, full, its KV launched) under `parent` with these ids; returns the cached page now holding the key,
-  // referenced once more: p itself, or the page cached before it
+  // page p (held by the caller, full, its KV launched) under `parent` with these ids; returns the cached page now holding
+  // the key: p itself, or the page cached before it, which the caller then holds as well
   int32_t publish(int32_t parent, const int32_t* ids, uint32_t depth, int32_t p) {
     Key k{parent, {}};
     std::copy(ids, ids + kPageTokens, k.ids.begin());
     auto ins = index.emplace(k, p);
     const int32_t q = ins.first->second;
-    if (!ins.second) { ref(q); return q; }
+    if (!ins.second) { if (q != p) ref(q); return q; }
     Node& n = node[p];
+    const uint32_t held = n.refs;
     n = Node{};
-    n.key = ins.first; n.cached = true; n.refs = 1; n.depth = depth;
+    n.key = ins.first; n.cached = true; n.refs = held; n.depth = depth;
     if (parent >= 0) node[parent].children++;
     published++;
     return p;
@@ -423,7 +449,7 @@ struct PrefixCache {
     evicted++;
     return p;
   }
-  // every page back to `free` (none may be held), in page order
+  // every cached page back to `free` (none may be held), in page order
   void clear(std::vector<int32_t>* free) {
     for (int32_t p = 0; p < int32_t(node.size()); ++p)
       if (node[p].cached) free->push_back(p);
@@ -490,6 +516,7 @@ struct llmlb_engine {
   // per-step metadata (device) + pinned staging ring
   int32_t *d_ids = nullptr, *d_pos = nullptr, *d_page_of_tok = nullptr, *d_tiles = nullptr,
           *d_last_rows = nullptr;
+  int32_t* d_fork_pages = nullptr;   // [max_seqs] the private tail pages of the choices a prefill step forks (kv_fork.cu)
   SlotState S{};
   BatchView B{};
   // penalties: int32 token counts [max_seqs][vocab] and bias lists [max_seqs][LLMLB_MAX_LOGIT_BIAS] per slot, and the
@@ -622,10 +649,13 @@ struct llmlb_engine {
   // fake CUDA runtime: heap-use-after-free in finish_request on cancel of a released, running request)
   void finish_request(ReqPtr r, uint32_t reason);
   void release_resources(ReqPtr r, bool publish = true);
-  // a page for new KV: the free pool first, then the least recently released evictable cached page (mu held)
+  // a page for new KV, held by the caller: the free pool first, then the least recently released evictable cached page
+  // (mu held)
   bool take_page(int32_t* p) {
-    if (!free_pages.empty()) { *p = free_pages.back(); free_pages.pop_back(); return true; }
-    return (*p = pc.evict()) >= 0;
+    if (!free_pages.empty()) { *p = free_pages.back(); free_pages.pop_back(); }
+    else if ((*p = pc.evict()) < 0) return false;
+    pc.node[*p].refs = 1;
+    return true;
   }
   size_t pages_available() const { return free_pages.size() + pc.lru.size(); }
   // the cached chain along r's context: at most (n - 1) / 64 pages, so at least one token is prefilled (mu held)
@@ -649,6 +679,17 @@ struct llmlb_engine {
       r.chain.push_back(pc.publish(j ? r.chain[j - 1] : -1, ids, j, r.pages[j]));
     }
   }
+  // a forking choice takes the group's full prompt pages (and the cached chain over them) beside its own tail page (mu held)
+  void share_prefix(const Request& head, Request& c, uint32_t n_full) {
+    std::vector<int32_t> own = std::move(c.pages);
+    c.pages.assign(head.pages.begin(), head.pages.begin() + n_full);
+    c.chain.assign(head.chain.begin(), head.chain.begin() + std::min<size_t>(head.chain.size(), n_full));
+    for (int32_t p : c.pages) pc.ref(p);
+    for (size_t j = 0; j < c.chain.size(); ++j)
+      if (c.chain[j] != c.pages[j]) pc.ref(c.chain[j]);
+    c.pages.insert(c.pages.end(), own.begin(), own.end());
+  }
+  void leave_group(const ReqPtr& r);
   void preempt(ReqPtr r);
   void expire_requests();     // leader / single rank: queue timeouts and request deadlines (time-based)
   std::atomic<uint64_t> preemptions{0};
@@ -729,7 +770,8 @@ int llmlb_engine::init() {
   LLMLB_CUDA_CHECK(cudaStreamSynchronize(st));
   if (tp == 1) RC(warmup());
   for (int32_t p = int32_t(n_pages) - 1; p >= 0; --p) free_pages.push_back(p);
-  if (cfg.prefix_cache) pc.node.resize(n_pages);
+  pc.node.resize(n_pages);   // holder counts of every page; the cache itself only with cfg.prefix_cache
+  pc.enabled = cfg.prefix_cache != 0;
   for (int32_t s = int32_t(cfg.max_seqs) - 1; s >= 0; --s) free_slots.push_back(s);
   worker = std::thread([this] { this->loop(); });
   return LLMLB_OK;
@@ -855,6 +897,7 @@ int llmlb_engine::alloc_all() {
   RC(dmalloc(&d_page_of_tok, t_cap));
   RC(dmalloc(&d_tiles, size_t(t_cap / 64 + cfg.max_seqs + 1) * 4));
   RC(dmalloc(&d_last_rows, cfg.max_seqs));
+  RC(dmalloc(&d_fork_pages, cfg.max_seqs));
   const size_t ms = cfg.max_seqs;
   RC(dmalloc(&S.seq_len, ms)); RC(dmalloc(&S.last_token, ms)); RC(dmalloc(&S.temperature, ms));
   RC(dmalloc(&S.top_p, ms)); RC(dmalloc(&S.top_k, ms)); RC(dmalloc(&S.seed, ms)); RC(dmalloc(&S.step, ms));
@@ -869,7 +912,7 @@ int llmlb_engine::alloc_all() {
   RC(dmalloc(&B.seed, ms)); RC(dmalloc(&B.step, ms)); RC(dmalloc(&B.out_ids, ms));
   // run_prefill's layout: ids, positions, pages [t_cap each] | tiles [tiles_cap x 4] | rows, slots, lens [max_seqs each] |
   // prompt-record rows, targets, alternatives [t_cap each]
-  stage_bytes = size_t(t_cap) * 4 * 3 + size_t(t_cap / 64 + ms + 1) * 16 + ms * 4 * 3 + size_t(t_cap) * 4 * 3 + 256;
+  stage_bytes = size_t(t_cap) * 4 * 3 + size_t(t_cap / 64 + ms + 1) * 16 + ms * 4 * 4 + size_t(t_cap) * 4 * 3 + 256;
   for (int i = 0; i < kRing; ++i) {
     LLMLB_CUDA_CHECK(cudaHostAlloc((void**)&h_stage[i], stage_bytes, cudaHostAllocDefault));
     LLMLB_CUDA_CHECK(cudaHostAlloc((void**)&h_out[i], ms * 4, cudaHostAllocDefault));
@@ -1275,36 +1318,49 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
   int32_t* s_slots = s_rows + cfg.max_seqs;
   int32_t* s_lens = s_slots + cfg.max_seqs;
   int32_t* s_plp = s_lens + cfg.max_seqs;   // prompt records: rows | targets | alternatives, t_cap apart (as d_plp_rows)
+  int32_t* s_fork = s_plp + size_t(t_cap) * 3;   // the forked choices' tail pages, group after group (as d_fork_pages)
 
   InflightStep step;
   step.is_prefill = true;
   step.n_tokens = T;
-  uint32_t row = 0, n_tiles = 0, R = 0, n_plp = 0;
+  uint32_t row = 0, n_tiles = 0, R = 0, n_plp = 0, n_fork = 0;
   bool pen_rows = false;   // some finished row is penalised
   bool lp_rows = false;    // some finished row reports logprobs
+  struct Fork { int32_t src; uint32_t off, n, rows; };   // kv_fork of a group's tail page into s_fork[off..off+n)
+  std::vector<Fork> forks;
+  std::vector<ReqPtr> forked;   // the choices this step forks off their group's prefill (not in reqs)
+  // first chunk of an admission (and a forking choice): publish block table + sampler state
+  auto slot_setup = [&](Request& r) -> int {
+    LLMLB_CUDA_CHECK(cudaMemcpyAsync(d_block_tables + size_t(r.slot) * pages_per_seq, r.pages.data(),
+                                     r.pages.size() * 4, cudaMemcpyHostToDevice, st));
+    slot_init_kernel<<<1, 1, 0, st>>>(S, r.slot, r.s.temperature, r.s.top_p, (int32_t)r.s.top_k, r.s.seed, uint64_t(r.harvested),
+                                 r.top_logprobs);
+    LLMLB_LAUNCH_CHECK();
+    if (r.penalized) {   // bias list into the slot's rows; counts = the tokens generated before a preemption (none otherwise)
+      const uint32_t nb = uint32_t(r.bias_ids.size());
+      if (nb) {
+        LLMLB_CUDA_CHECK(cudaMemcpyAsync(pen_bias_ids + size_t(r.slot) * LLMLB_MAX_LOGIT_BIAS, r.bias_ids.data(), nb * 4, cudaMemcpyHostToDevice, st));
+        LLMLB_CUDA_CHECK(cudaMemcpyAsync(pen_bias_vals + size_t(r.slot) * LLMLB_MAX_LOGIT_BIAS, r.bias_vals.data(), nb * 4, cudaMemcpyHostToDevice, st));
+      }
+      if (!r.gen.empty()) LLMLB_CUDA_CHECK(cudaMemcpyAsync(pen_gen, r.gen.data(), r.gen.size() * 4, cudaMemcpyHostToDevice, st));
+      RC(penalty_reset_launch(pen_counts, M.vocab, S.pen_freq, S.pen_pres, S.pen_n_bias, r.slot, r.freq_pen, r.pres_pen, nb,
+                              M.vocab, pen_gen, uint32_t(r.gen.size()), st));
+    }
+    r.pages_published = uint32_t(r.pages.size());
+    return LLMLB_OK;
+  };
   for (size_t i = 0; i < reqs.size(); ++i) {
     Request& r = *reqs[i];
-    if (r.pages_published == 0) {  // first chunk of this admission: publish block table + sampler state
-      LLMLB_CUDA_CHECK(cudaMemcpyAsync(d_block_tables + size_t(r.slot) * pages_per_seq, r.pages.data(),
-                                       r.pages.size() * 4, cudaMemcpyHostToDevice, st));
-      slot_init_kernel<<<1, 1, 0, st>>>(S, r.slot, r.s.temperature, r.s.top_p, (int32_t)r.s.top_k, r.s.seed, uint64_t(r.harvested),
-                                   r.top_logprobs);
-      LLMLB_LAUNCH_CHECK();
-      if (r.penalized) {   // bias list into the slot's rows; counts = the tokens generated before a preemption (none otherwise)
-        const uint32_t nb = uint32_t(r.bias_ids.size());
-        if (nb) {
-          LLMLB_CUDA_CHECK(cudaMemcpyAsync(pen_bias_ids + size_t(r.slot) * LLMLB_MAX_LOGIT_BIAS, r.bias_ids.data(), nb * 4, cudaMemcpyHostToDevice, st));
-          LLMLB_CUDA_CHECK(cudaMemcpyAsync(pen_bias_vals + size_t(r.slot) * LLMLB_MAX_LOGIT_BIAS, r.bias_vals.data(), nb * 4, cudaMemcpyHostToDevice, st));
-        }
-        if (!r.gen.empty()) LLMLB_CUDA_CHECK(cudaMemcpyAsync(pen_gen, r.gen.data(), r.gen.size() * 4, cudaMemcpyHostToDevice, st));
-        RC(penalty_reset_launch(pen_counts, M.vocab, S.pen_freq, S.pen_pres, S.pen_n_bias, r.slot, r.freq_pen, r.pres_pen, nb,
-                                M.vocab, pen_gen, uint32_t(r.gen.size()), st));
-      }
-      r.pages_published = uint32_t(r.pages.size());
-    }
+    if (r.pages_published == 0) RC(slot_setup(r));
     const uint32_t p0 = r.prefilled;
-    for (uint32_t pg = p0 / kPageTokens; pc.on() && pg <= (p0 + take[i] - 1) / kPageTokens; ++pg)
-      if (pc.shared(r.pages[pg])) { set_error("prefix cache: a prefill step would write into a cached page"); return LLMLB_E_INTERNAL; }
+    for (uint32_t pg = p0 / kPageTokens; pg <= (p0 + take[i] - 1) / kPageTokens; ++pg)
+      if (pc.shared(r.pages[pg])) {
+        set_error(pc.node[r.pages[pg]].cached ? "prefix cache: a prefill step would write into a cached page"
+                                             : "a prefill step would write into a page another sequence holds");
+        return LLMLB_E_INTERNAL;
+      }
+    // the group's choices, the prefilling one first, when this chunk completes their prompt (the one request otherwise)
+    const std::vector<ReqPtr> members = p0 + take[i] == r.prompt.size() ? group_members(reqs[i]) : std::vector<ReqPtr>{reqs[i]};
     for (uint32_t j = 0; j < take[i]; ++j) {
       uint32_t pos = p0 + j;
       s_ids[row + j] = r.prompt[pos];
@@ -1316,7 +1372,8 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
       // the chunk's positions that have a next prompt token and were not reported before a preemption (which happens with
       // nothing in flight, so prompt_lp_done is exact then; within one admission the chunks are disjoint)
       const uint32_t lo = std::max(p0, r.prompt_lp_done), hi = std::min(p0 + take[i], r.n_prompt0 - 1);
-      if (lo < hi) step.prompt_lp.push_back({reqs[i], lo, hi - lo, n_plp});
+      if (lo < hi)   // computed once, delivered to every choice of a group
+        for (const ReqPtr& m : group_members(reqs[i])) step.prompt_lp.push_back({m, lo, hi - lo, n_plp});
       for (uint32_t p = lo; p < hi; ++p, ++n_plp) {
         s_plp[n_plp] = int32_t(row + p - p0);
         s_plp[t_cap + n_plp] = r.prompt[p + 1];   // the target of a chunk's last row lies in the next chunk
@@ -1324,16 +1381,33 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
       }
     }
     if (p0 + take[i] == r.prompt.size()) {
-      s_rows[R] = int32_t(row + take[i] - 1);
-      s_slots[R] = r.slot;
-      s_lens[R] = int32_t(r.prompt.size());
-      pen_rows |= r.penalized;
-      lp_rows |= r.top_logprobs >= 0;
-      step.reqs.push_back(reqs[i]);
-      ++R;
+      // the fork: the other choices take the full prompt pages, their tail pages get a copy of the prompt's last rows
+      // (after this step's forward wrote them), and every choice samples its first token from the same last row
+      const uint32_t L = uint32_t(r.prompt.size()), n_full = L / kPageTokens;
+      if (members.size() > 1) {
+        std::lock_guard<std::mutex> lk(mu);
+        for (size_t m = 1; m < members.size(); ++m) share_prefix(r, *members[m], n_full);
+        for (const ReqPtr& m : members) m->group.reset();
+      }
+      if (members.size() > 1 && L % kPageTokens) {
+        forks.push_back({r.pages[n_full], n_fork, uint32_t(members.size() - 1), L % kPageTokens});
+        for (size_t m = 1; m < members.size(); ++m) s_fork[n_fork++] = members[m]->pages[n_full];
+      }
+      for (size_t m = 0; m < members.size(); ++m) {
+        Request& c = *members[m];
+        if (m) { RC(slot_setup(c)); forked.push_back(members[m]); }
+        s_rows[R] = int32_t(row + take[i] - 1);
+        s_slots[R] = c.slot;
+        s_lens[R] = int32_t(L);
+        pen_rows |= c.penalized;
+        lp_rows |= c.top_logprobs >= 0;
+        step.reqs.push_back(members[m]);
+        ++R;
+      }
     }
     row += take[i];
   }
+  if (n_fork) LLMLB_CUDA_CHECK(cudaMemcpyAsync(d_fork_pages, s_fork, n_fork * 4, cudaMemcpyHostToDevice, st));
   // note: r.pages.data() above is pageable host memory: the async copy is staged by the driver
   LLMLB_CUDA_CHECK(cudaMemcpyAsync(d_ids, s_ids, T * 4, cudaMemcpyHostToDevice, st));
   LLMLB_CUDA_CHECK(cudaMemcpyAsync(d_pos, s_pos, T * 4, cudaMemcpyHostToDevice, st));
@@ -1363,6 +1437,8 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
     LLMLB_LAUNCH_CHECK();
     RC(copy_out(&step, R, lp_rows));
   }
+  for (const Fork& f : forks)
+    RC(kv_fork_launch(k_pool, v_pool, M.n_layers, n_pages, nkv_l, f.src, d_fork_pages + f.off, f.n, f.rows, st));
   // prompt records: the same lm_head path and logprob_kernel over the prompt rows, max_seqs rows at a time (the rows the
   // logits buffers hold); no penalties or bias: those act on generated tokens
   for (uint32_t g = 0; g < n_plp; g += cfg.max_seqs) {
@@ -1391,6 +1467,10 @@ int llmlb_engine::run_prefill(const std::vector<ReqPtr>& reqs, const std::vector
       reqs[i]->prefilled += take[i];
       if (reqs[i]->prefilled == reqs[i]->prompt.size()) reqs[i]->launched = reqs[i]->harvested + 1;
       if (pc.on()) pc_publish(*reqs[i], reqs[i]->prefilled);   // later steps that read them are ordered after this one
+    }
+    for (const ReqPtr& c : forked) {
+      c->prefilled = uint32_t(c->prompt.size());
+      c->launched = c->harvested + 1;
     }
     steps_prefill++;
     tokens_prefill += T;
@@ -1426,11 +1506,14 @@ int llmlb_engine::run_decode(const std::vector<ReqPtr>& batch) {
       }
     }
   }
-  for (auto& r : batch)   // the page that receives the input token's KV
-    if (pc.shared(r->pages[(r->n_prompt0 + r->launched - 1) / kPageTokens])) {
-      set_error("prefix cache: a decode step would write into a cached page");
+  for (auto& r : batch) {   // the page that receives the input token's KV
+    const int32_t p = r->pages[(r->n_prompt0 + r->launched - 1) / kPageTokens];
+    if (pc.shared(p)) {
+      set_error(pc.node[p].cached ? "prefix cache: a decode step would write into a cached page"
+                                  : "a decode step would write into a page another sequence holds");
       return LLMLB_E_INTERNAL;
     }
+  }
   InflightStep step;
   step.n_tokens = nb;
   step.reqs = batch;
@@ -1453,8 +1536,8 @@ int llmlb_engine::run_decode(const std::vector<ReqPtr>& batch) {
 }
 
 // publish: cache the full pages whose every position was the input of a launched step (prefilled context, and generated
-// tokens that a harvested token followed: in-flight steps only write positions beyond those).  Duplicates and private
-// pages go back to the free pool, cached ones are released.
+// tokens that a harvested token followed: in-flight steps only write positions beyond those).  Then r lets go of every page
+// it holds: one that nobody else holds goes back to the free pool if it is not cached, and becomes evictable if it is.
 void llmlb_engine::release_resources(ReqPtr r, bool publish) {  // mu held
   if (r->slot >= 0) {
     free_slots.push_back(r->slot);
@@ -1464,11 +1547,12 @@ void llmlb_engine::release_resources(ReqPtr r, bool publish) {  // mu held
     uint32_t limit = r->prefilled;
     if (r->prefilled == r->prompt.size() && r->harvested > 0) limit = std::max(limit, r->n_prompt0 + r->harvested - 1);
     if (publish) pc_publish(*r, limit);
-    pc.tick++;
-    for (int32_t p : r->chain) pc.unref(p);
   }
-  for (size_t j = 0; j < r->pages.size(); ++j)
-    if (j >= r->chain.size() || r->chain[j] != r->pages[j]) free_pages.push_back(r->pages[j]);
+  pc.tick++;
+  for (int32_t p : r->pages)
+    if (pc.unref(p)) free_pages.push_back(p);
+  for (size_t j = 0; j < r->chain.size(); ++j)   // the cached duplicates of private pages
+    if (r->chain[j] != r->pages[j]) pc.unref(r->chain[j]);
   r->chain.clear();
   r->pages.clear();
   r->pages_published = 0;
@@ -1496,8 +1580,28 @@ static llmlb_token_logprobs no_logprobs() {
   return lp;
 }
 
+// r leaves its group before the fork (it finishes).  If r was prefilling the prompt, the next choice takes over r's pages,
+// cached chain and prefill progress and continues from its own slot; r keeps that choice's tail page.  mu held.
+void llmlb_engine::leave_group(const ReqPtr& r) {
+  if (!r->group) return;
+  auto& g = *r->group;
+  const bool prefilling = g.front().lock() == r;
+  g.erase(std::remove_if(g.begin(), g.end(), [&](const std::weak_ptr<Request>& w) { return w.lock() == r; }), g.end());
+  if (prefilling && !g.empty() && r->slot >= 0) {
+    const ReqPtr h = g.front().lock();
+    std::swap(h->pages, r->pages);
+    std::swap(h->chain, r->chain);
+    h->prefilled = r->prefilled;
+    h->pages_published = 0;   // its next chunk publishes the block table and sampler state of its slot
+    r->prefilled = 0;
+  }
+  if (g.size() == 1) g.front().lock()->group.reset();   // a group of one is a lone request
+  r->group.reset();
+}
+
 void llmlb_engine::finish_request(ReqPtr r, uint32_t reason) {  // mu held
   if (r->finished) return;
+  leave_group(r);
   r->finished = true;
   r->finish_reason = reason;
   if (r->events.empty() || r->events.back().finish_reason == LLMLB_FINISH_NONE) {
@@ -1593,7 +1697,7 @@ bool llmlb_engine::sched_iteration(std::unique_lock<std::mutex>& lk) {
     // continue chunked prefills first
     for (auto& r : running) {
       if (budget == 0) break;
-      if (r->prefilled < r->prompt.size()) {
+      if (r->prefilled < r->prompt.size() && !awaits_fork(*r)) {
         uint32_t t = std::min<uint32_t>(budget, (uint32_t)r->prompt.size() - r->prefilled);
         pf_reqs.push_back(r); pf_take.push_back(t); budget -= t;
       }
@@ -1603,12 +1707,18 @@ bool llmlb_engine::sched_iteration(std::unique_lock<std::mutex>& lk) {
     // time as a sequence crosses a page boundary; when the pool runs dry the most recently admitted
     // sequence is evicted and recomputed later (below).
     // With the prefix cache the context's cached chain comes first and needs no new page; evictable pages count as free.
+    // The n choices of a group (at the head of the queue, in choice order) are admitted together: n slots, one lookup, and
+    // a private tail page for every choice but the first when the prompt ends inside a page.
     std::vector<int32_t> hit;
     while (!waiting.empty() && budget > 0 && !free_slots.empty()) {
       ReqPtr r = waiting.front();
+      const std::vector<ReqPtr> members = group_members(r);
+      const uint32_t k = uint32_t(members.size());
+      if (free_slots.size() < k) break;
       hit.clear();
       if (pc.on() && !r->prompt_lp) pc_match(*r, &hit);   // prompt records need every prompt row's logits
-      uint32_t need = ceil_div((uint32_t)r->prompt.size(), kPageTokens) - uint32_t(hit.size());
+      const uint32_t tails = (k - 1) * ((uint32_t)r->prompt.size() % kPageTokens != 0);
+      uint32_t need = ceil_div((uint32_t)r->prompt.size(), kPageTokens) - uint32_t(hit.size()) + tails;
       size_t avail = pages_available();
       for (int32_t p : hit) avail -= pc.node[p].refs == 0;   // a matched evictable page stops being evictable
       // first admission keeps one page per running sequence in reserve, so that admitting does not
@@ -1626,9 +1736,18 @@ bool llmlb_engine::sched_iteration(std::unique_lock<std::mutex>& lk) {
         r->prefilled = uint32_t(hit.size()) * kPageTokens;
         if (!r->admitted_once) r->cached_tokens = std::min(r->prefilled, r->n_prompt0);
       }
-      for (uint32_t i = 0; i < need; ++i) { int32_t p; take_page(&p); r->pages.push_back(p); }
+      for (uint32_t i = 0; i < need - tails; ++i) { int32_t p; take_page(&p); r->pages.push_back(p); }
       r->admitted_once = true;
       running.push_back(r);
+      for (uint32_t m = 1; m < k; ++m) {   // the other choices wait for the fork
+        const ReqPtr& c = members[m];
+        waiting.erase(std::find(waiting.begin(), waiting.end(), c));   // submitted together, right behind r
+        c->slot = free_slots.back(); free_slots.pop_back();
+        if (tails) { int32_t p; take_page(&p); c->pages.push_back(p); }
+        c->cached_tokens = r->cached_tokens;
+        c->admitted_once = true;
+        running.push_back(c);
+      }
       uint32_t t = std::min<uint32_t>(budget, (uint32_t)r->prompt.size() - r->prefilled);
       pf_reqs.push_back(r); pf_take.push_back(t); budget -= t;
     }
@@ -1738,9 +1857,13 @@ void llmlb_engine::loop_follower() {
     const uint32_t type = plan.read(&buf, plan_abort);
     if (type == 0 || type == kPlanStop) break;
     switch (type) {
-      case kPlanSubmit: {
-        if (buf.size() < sizeof(uint64_t) + sizeof(llmlb_sampling) + 8) break;
+      case kPlanSubmit:
+      case kPlanSubmitChoices: {
+        uint32_t n_choices = 1;
+        const size_t pre = type == kPlanSubmitChoices ? 8 : 0;
+        if (buf.size() < pre + sizeof(uint64_t) + sizeof(llmlb_sampling) + 8) break;
         const uint8_t* p = buf.data();
+        if (pre) { memcpy(&n_choices, p, 4); p += pre; }
         auto r = std::make_shared<Request>();
         memcpy(&r->id, p, 8); p += 8;
         memcpy(&r->s, p, sizeof(llmlb_sampling)); p += sizeof(llmlb_sampling);
@@ -1768,6 +1891,15 @@ void llmlb_engine::loop_follower() {
         std::lock_guard<std::mutex> lk(mu);
         requests[r->id] = r;
         waiting.push_back(r);
+        if (n_choices > 1) r->group = std::make_shared<std::vector<std::weak_ptr<Request>>>(1, r);
+        for (uint32_t i = 1; i < n_choices; ++i) {   // as submit_request builds a group
+          auto c = std::make_shared<Request>(*r);
+          c->id = r->id + i;
+          c->s.seed = r->s.seed + i;
+          c->group->push_back(c);
+          requests[c->id] = c;
+          waiting.push_back(c);
+        }
         break;
       }
       case kPlanCancel:
@@ -1850,7 +1982,7 @@ extern "C" void llmlb_engine_destroy(llmlb_engine* e) {
   for (auto& L : e->layers) { F(L.wqkv); F(L.wo); F(L.wgu); F(L.wdown); F(L.attn_norm); F(L.ffn_norm); }
   F(e->k_pool); F(e->v_pool); F(e->rope); F(e->d_block_tables);
   F(e->x); if (e->tp == 1) F(e->y); F(e->xb); F(e->tp_stage); F(e->ylast); F(e->qkv); F(e->attn); F(e->h); F(e->logits); F(e->logits_l); F(e->x_last); F(e->attn_ws);
-  F(e->d_ids); F(e->d_pos); F(e->d_page_of_tok); F(e->d_tiles); F(e->d_last_rows);
+  F(e->d_ids); F(e->d_pos); F(e->d_page_of_tok); F(e->d_tiles); F(e->d_last_rows); F(e->d_fork_pages);
   F(e->S.seq_len); F(e->S.last_token); F(e->S.temperature); F(e->S.top_p); F(e->S.top_k); F(e->S.seed); F(e->S.step);
   F(e->S.pen_freq); F(e->S.pen_pres); F(e->S.pen_n_bias); F(e->pen_counts); F(e->pen_bias_ids); F(e->pen_bias_vals); F(e->pen_gen);
   F(e->S.lp_top); F(e->d_lp); F(e->d_plp_rows); F(e->d_plp);
@@ -1958,7 +2090,8 @@ static int take_penalties(const llmlb_penalties* pen, uint32_t vocab, Request* r
 }
 
 static int submit_request(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt, const llmlb_sampling* s,
-                          const llmlb_penalties* pen, int32_t top_logprobs, bool prompt_lp, uint64_t* req_id, const char* bad_arg);
+                          const llmlb_penalties* pen, int32_t top_logprobs, bool prompt_lp, uint64_t* req_id, const char* bad_arg,
+                          uint32_t n_choices = 1);
 
 extern "C" int llmlb_request_submit(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt,
                                     const llmlb_sampling* s, uint64_t* req_id) {
@@ -1993,9 +2126,28 @@ extern "C" int llmlb_request_submit_prompt_logprobs(llmlb_engine* e, const int32
                         "llmlb_request_submit_prompt_logprobs: bad argument");
 }
 
-// top_logprobs: -1 = the request reports no logprobs; prompt_lp (with top_logprobs >= 0): also its prompt records
+extern "C" int llmlb_request_submit_choices(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt, const llmlb_sampling* s,
+                                            const llmlb_penalties* pen, int32_t top_logprobs, uint32_t prompt_logprobs, uint32_t n,
+                                            uint64_t* req_ids) {
+  const char* fn = "llmlb_request_submit_choices: ";
+  if (e && (n == 0 || n > e->cfg.max_seqs)) {
+    set_error(std::string(fn) + "n must be in [1, max_seqs = " + std::to_string(e->cfg.max_seqs) + "], got " + std::to_string(n));
+    return LLMLB_E_INVALID_ARG;
+  }
+  if (top_logprobs < -1 || top_logprobs > int32_t(LLMLB_MAX_TOP_LOGPROBS)) {
+    set_error(std::string(fn) + "top_logprobs must be -1 (none) or in [0, 20]");
+    return LLMLB_E_INVALID_ARG;
+  }
+  if (prompt_logprobs && top_logprobs < 0) { set_error(std::string(fn) + "prompt_logprobs needs top_logprobs >= 0"); return LLMLB_E_INVALID_ARG; }
+  return submit_request(e, prompt_ids, n_prompt, s, pen, top_logprobs, prompt_logprobs != 0, req_ids,
+                        "llmlb_request_submit_choices: bad argument", n);
+}
+
+// top_logprobs: -1 = the request reports no logprobs; prompt_lp (with top_logprobs >= 0): also its prompt records.
+// n_choices > 1: a group (llmlb_request_submit_choices), ids into req_id[0 .. n_choices)
 static int submit_request(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n_prompt, const llmlb_sampling* s,
-                          const llmlb_penalties* pen, int32_t top_logprobs, bool prompt_lp, uint64_t* req_id, const char* bad_arg) {
+                          const llmlb_penalties* pen, int32_t top_logprobs, bool prompt_lp, uint64_t* req_id, const char* bad_arg,
+                          uint32_t n_choices) {
   if (!e || !prompt_ids || !s || !req_id || n_prompt == 0) {
     set_error(bad_arg);
     return LLMLB_E_INVALID_ARG;
@@ -2024,18 +2176,33 @@ static int submit_request(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n
     std::lock_guard<std::mutex> lk(e->mu);
     if (e->plan_on && !e->plan.leader) { set_error("follower rank of a plan channel: requests enter through rank 0"); return LLMLB_E_UNSUPPORTED; }
     if (!e->fatal_error.empty()) { set_error("engine failed: " + e->fatal_error); return LLMLB_E_DEVICE; }
-    if (e->waiting.size() >= (e->cfg.queue_max ? e->cfg.queue_max : 4096u)) { set_error("Request queue is full"); return LLMLB_E_QUEUE_FULL; }
+    if (e->waiting.size() + n_choices > (e->cfg.queue_max ? e->cfg.queue_max : 4096u)) { set_error("Request queue is full"); return LLMLB_E_QUEUE_FULL; }
     r->id = e->next_id++;
     e->served = true;
     e->requests[r->id] = r;
     e->waiting.push_back(r);
     *req_id = r->id;
+    if (n_choices > 1) {   // choice i: the same request with seed + i (wrapping), queued right behind choice i - 1
+      r->group = std::make_shared<std::vector<std::weak_ptr<Request>>>(1, r);
+      for (uint32_t i = 1; i < n_choices; ++i) {
+        auto c = std::make_shared<Request>(*r);
+        c->id = e->next_id++;
+        c->s.seed = r->s.seed + i;
+        c->group->push_back(c);
+        e->requests[c->id] = c;
+        e->waiting.push_back(c);
+        req_id[i] = c->id;
+      }
+    }
     if (e->plan_on) {   // id, sampling, prompt, stop ids, (penalised requests) the penalties, (logprob requests)
                         // top_logprobs and (prompt logprobs) the prompt flag travel to the followers in queue order
       const uint32_t n_bias = uint32_t(r->bias_ids.size());
-      std::vector<uint8_t> rec(8 + sizeof(llmlb_sampling) + 8 + (size_t(n_prompt) + r->stop_ids.size()) * 4 +
+      // a group: [u32 n][u32 0] first, and the record of choice 0
+      const size_t pre = n_choices > 1 ? 8 : 0;
+      std::vector<uint8_t> rec(pre + 8 + sizeof(llmlb_sampling) + 8 + (size_t(n_prompt) + r->stop_ids.size()) * 4 +
                                (r->penalized ? 12 + size_t(n_bias) * 8 : 0) + (top_logprobs >= 0 ? 4 : 0) + (prompt_lp ? 4 : 0));
       uint8_t* p = rec.data();
+      if (pre) { memcpy(p, &n_choices, 4); p += pre; }
       memcpy(p, &r->id, 8); p += 8;
       memcpy(p, &r->s, sizeof(llmlb_sampling)); p += sizeof(llmlb_sampling);
       const uint32_t n_stop = uint32_t(r->stop_ids.size());
@@ -2052,7 +2219,7 @@ static int submit_request(llmlb_engine* e, const int32_t* prompt_ids, uint32_t n
       // least 12)
       if (top_logprobs >= 0) memcpy(p, &top_logprobs, 4);
       if (prompt_lp) { const uint32_t one = 1; memcpy(p + 4, &one, 4); }
-      e->plan_log(kPlanSubmit, rec.data(), uint32_t(rec.size()));
+      e->plan_log(pre ? kPlanSubmitChoices : kPlanSubmit, rec.data(), uint32_t(rec.size()));
     }
   }
   e->cv_sched.notify_all();

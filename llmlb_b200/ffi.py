@@ -104,6 +104,7 @@ PROTOTYPES = {
     "llmlb_request_submit_prompt_logprobs": (C.c_int, [vp, _P(i32), u32, _P(Sampling), _P(Penalties), u32, _P(u64)]),
     "llmlb_request_poll_prompt_logprobs": (C.c_int, [vp, u64, _P(TokenLogprobs), u32, _P(u32)]),
     "llmlb_request_cached_tokens": (C.c_int, [vp, u64, _P(u32)]),
+    "llmlb_request_submit_choices": (C.c_int, [vp, _P(i32), u32, _P(Sampling), _P(Penalties), i32, u32, u32, _P(u64)]),
     "llmlb_request_cancel": (C.c_int, [vp, u64]),
     "llmlb_request_release": (C.c_int, [vp, u64]),
     "llmlb_debug_prefill_logits": (C.c_int, [vp, _P(i32), u32, _P(f32), _P(f32)]),
@@ -129,6 +130,7 @@ PROTOTYPES = {
     "llmlb_op_penalize": (C.c_int, [vp, u32, u32, vp, u64, vp, vp, vp, vp, vp, u32, vp]),
     "llmlb_op_logprobs": (C.c_int, [vp, u32, u32, vp, vp, vp, vp]),
     "llmlb_op_allreduce": (C.c_int, [vp, vp, u64, vp]),
+    "llmlb_op_kv_fork": (C.c_int, [vp, vp, u32, u32, u32, i32, vp, u32, u32, vp]),
     "llmlb_op_synth_bf16": (C.c_int, [vp, u64, u64, u64, u64, u64, u64, u32, f32, vp]),
 }
 
@@ -277,6 +279,34 @@ class Engine:
         else:
             check(submit_lp(self._h, arr, n, C.byref(s), C.byref(pen), int(logprobs), C.byref(rid)))
         return rid.value
+
+    def submit_choices(self, prompt_ids, max_tokens, n, temperature=0.0, top_k=0, top_p=1.0, seed=0, stop_ids=(),
+                       ignore_eos=False, frequency_penalty=None, presence_penalty=None, logit_bias=None, logprobs=None,
+                       prompt_logprobs=False):
+        """OpenAI's n: n choices of one prompt through llmlb_request_submit_choices (one prefill, then a fork of its KV
+        pages); returns the n request ids, choice i sampling with seed + i.  The other arguments are submit's."""
+        if prompt_logprobs and logprobs is None:
+            raise ValueError("prompt_logprobs needs logprobs (the number of alternatives)")
+        arr = (i32 * len(prompt_ids))(*prompt_ids)
+        s = Sampling()
+        s.max_tokens, s.temperature, s.top_k, s.top_p, s.seed = max_tokens, temperature, top_k, top_p, seed
+        stops = (i32 * max(1, len(stop_ids)))(*stop_ids)
+        s.stop_ids = C.cast(stops, _P(i32)) if stop_ids else None
+        s.n_stop_ids = len(stop_ids)
+        s.ignore_eos = 1 if ignore_eos else 0
+        pen = None
+        if frequency_penalty is not None or presence_penalty is not None or logit_bias is not None:
+            bias = list((logit_bias or {}).items())
+            ids = (i32 * max(1, len(bias)))(*[int(k) for k, _ in bias])
+            vals = (f32 * max(1, len(bias)))(*[float(v) for _, v in bias])
+            pen = Penalties()
+            pen.frequency_penalty = frequency_penalty or 0.0
+            pen.presence_penalty = presence_penalty or 0.0
+            pen.bias_ids, pen.bias_values, pen.n_bias = C.cast(ids, _P(i32)), C.cast(vals, _P(f32)), len(bias)
+        rids = (u64 * max(1, n))()
+        check(lib().llmlb_request_submit_choices(self._h, arr, len(prompt_ids), C.byref(s), C.byref(pen) if pen else None,
+                                                 -1 if logprobs is None else int(logprobs), 1 if prompt_logprobs else 0, n, rids))
+        return list(rids[:n])
 
     def poll(self, rid, cap=256, timeout_ms=0):
         buf = (TokenEvent * cap)()

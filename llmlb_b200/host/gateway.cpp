@@ -517,12 +517,13 @@ std::string sha256_hex(const std::string& data) {
 std::string sse_event(const Json& j) { return "data: " + j.dump() + "\n\n"; }
 
 Json chat_chunk(const std::string& id, const std::string& model, int64_t created,
-                const std::string* role, const std::string* content, const char* finish_reason, const Json* logprobs) {
+                const std::string* role, const std::string* content, const char* finish_reason, const Json* logprobs,
+                uint32_t index) {
   Json delta = Json::object();
   if (role) delta.set("role", *role);
   if (content) delta.set("content", *content);
   Json choice = Json::object();
-  choice.set("index", 0); choice.set("delta", delta);
+  choice.set("index", index); choice.set("delta", delta);
   if (logprobs) choice.set("logprobs", *logprobs);
   choice.set("finish_reason", finish_reason ? Json(finish_reason) : Json());
   Json root = Json::object();
@@ -552,12 +553,19 @@ Json chat_usage_chunk(const std::string& id, const std::string& model, int64_t c
 Json chat_completion_body(const std::string& id, const std::string& model, int64_t created,
                           const std::string& content, const char* finish_reason, uint32_t p, uint32_t c, const Json* logprobs,
                           const uint32_t* cached) {
-  Json msg = Json::object(); msg.set("role", "assistant"); msg.set("content", content);
-  Json choice = Json::object();
-  choice.set("index", 0); choice.set("message", msg);
-  if (logprobs) choice.set("logprobs", *logprobs);
-  choice.set("finish_reason", finish_reason ? Json(finish_reason) : Json());
-  Json choices = Json::array(); choices.push(choice);
+  return chat_completion_body(id, model, created, std::vector<ChoiceOut>{{content, finish_reason, logprobs}}, p, c, cached);
+}
+Json chat_completion_body(const std::string& id, const std::string& model, int64_t created, const std::vector<ChoiceOut>& outs,
+                          uint32_t p, uint32_t c, const uint32_t* cached) {
+  Json choices = Json::array();
+  for (size_t i = 0; i < outs.size(); ++i) {
+    Json msg = Json::object(); msg.set("role", "assistant"); msg.set("content", outs[i].text);
+    Json choice = Json::object();
+    choice.set("index", uint32_t(i)); choice.set("message", msg);
+    if (outs[i].logprobs) choice.set("logprobs", *outs[i].logprobs);
+    choice.set("finish_reason", outs[i].finish_reason ? Json(outs[i].finish_reason) : Json());
+    choices.push(choice);
+  }
   Json root = Json::object();
   root.set("id", id); root.set("object", "chat.completion"); root.set("created", created); root.set("model", model);
   root.set("choices", choices); root.set("usage", chat_usage(p, c, cached));
@@ -566,20 +574,27 @@ Json chat_completion_body(const std::string& id, const std::string& model, int64
 Json completion_body(const std::string& id, const std::string& model, int64_t created,
                      const std::string& text, const char* finish_reason, uint32_t p, uint32_t c, const Json* logprobs,
                      const uint32_t* cached) {
-  Json choice = Json::object();
-  choice.set("index", 0); choice.set("text", text);
-  if (logprobs) choice.set("logprobs", *logprobs);
-  choice.set("finish_reason", finish_reason ? Json(finish_reason) : Json());
-  Json choices = Json::array(); choices.push(choice);
+  return completion_body(id, model, created, std::vector<ChoiceOut>{{text, finish_reason, logprobs}}, p, c, cached);
+}
+Json completion_body(const std::string& id, const std::string& model, int64_t created, const std::vector<ChoiceOut>& outs,
+                     uint32_t p, uint32_t c, const uint32_t* cached) {
+  Json choices = Json::array();
+  for (size_t i = 0; i < outs.size(); ++i) {
+    Json choice = Json::object();
+    choice.set("index", uint32_t(i)); choice.set("text", outs[i].text);
+    if (outs[i].logprobs) choice.set("logprobs", *outs[i].logprobs);
+    choice.set("finish_reason", outs[i].finish_reason ? Json(outs[i].finish_reason) : Json());
+    choices.push(choice);
+  }
   Json root = Json::object();
   root.set("id", id); root.set("object", "text_completion"); root.set("created", created); root.set("model", model);
   root.set("choices", choices); root.set("usage", chat_usage(p, c, cached));
   return root;
 }
 Json completion_chunk(const std::string& id, const std::string& model, int64_t created, const std::string* text, const char* finish_reason,
-                      const Json* logprobs) {
+                      const Json* logprobs, uint32_t index) {
   Json choice = Json::object();
-  choice.set("index", 0); choice.set("text", text ? *text : std::string()); choice.set("logprobs", logprobs ? *logprobs : Json());
+  choice.set("index", index); choice.set("text", text ? *text : std::string()); choice.set("logprobs", logprobs ? *logprobs : Json());
   choice.set("finish_reason", finish_reason ? Json(finish_reason) : Json());
   Json choices = Json::array(); choices.push(choice);
   Json root = Json::object();

@@ -259,23 +259,35 @@ inline std::string sse_done() { return "data: [DONE]\n\n"; }
 // logprobs (optional): the choice's "logprobs" value (chat_logprobs / completion_logprobs); without it the shapes are the
 // ones above, byte for byte.  cached_tokens (optional, a prefix-cache engine): usage gains
 // "prompt_tokens_details":{"cached_tokens":N} ("input_tokens_details" on responses); without it usage is unchanged
+// index: the choice a chunk carries (OpenAI's n; 0 = the only one)
 Json chat_chunk(const std::string& id, const std::string& model, int64_t created,
                 const std::string* role, const std::string* content, const char* finish_reason,
-                const Json* logprobs = nullptr);
+                const Json* logprobs = nullptr, uint32_t index = 0);
 Json chat_usage_chunk(const std::string& id, const std::string& model, int64_t created,
                       uint32_t prompt_tokens, uint32_t completion_tokens, const uint32_t* cached_tokens = nullptr);
 Json chat_completion_body(const std::string& id, const std::string& model, int64_t created,
                           const std::string& content, const char* finish_reason,
                           uint32_t prompt_tokens, uint32_t completion_tokens, const Json* logprobs = nullptr,
                           const uint32_t* cached_tokens = nullptr);
+// One choice of a body with several (OpenAI's n): its text, finish reason and logprobs value (optional).  The one-choice
+// bodies above are these with a single choice, byte for byte.
+struct ChoiceOut {
+  std::string text;
+  const char* finish_reason = nullptr;
+  const Json* logprobs = nullptr;
+};
+Json chat_completion_body(const std::string& id, const std::string& model, int64_t created, const std::vector<ChoiceOut>& choices,
+                          uint32_t prompt_tokens, uint32_t completion_tokens, const uint32_t* cached_tokens = nullptr);
 // legacy /v1/completions stream: {"object":"text_completion","choices":[{"index":0,"text":...,"finish_reason":...}]}
 Json completion_chunk(const std::string& id, const std::string& model, int64_t created, const std::string* text, const char* finish_reason,
-                      const Json* logprobs = nullptr);
+                      const Json* logprobs = nullptr, uint32_t index = 0);
 Json completion_usage_chunk(const std::string& id, const std::string& model, int64_t created, uint32_t prompt_tokens, uint32_t completion_tokens,
                             const uint32_t* cached_tokens = nullptr);
 Json completion_body(const std::string& id, const std::string& model, int64_t created,
                      const std::string& text, const char* finish_reason, uint32_t prompt_tokens,
                      uint32_t completion_tokens, const Json* logprobs = nullptr, const uint32_t* cached_tokens = nullptr);
+Json completion_body(const std::string& id, const std::string& model, int64_t created, const std::vector<ChoiceOut>& choices,
+                     uint32_t prompt_tokens, uint32_t completion_tokens, const uint32_t* cached_tokens = nullptr);
 
 // ---- OpenAI logprobs ----
 // One listed token (or one of its alternatives): text through from_utf8_lossy, raw bytes, log-probability.

@@ -43,6 +43,7 @@
 #pragma weak llmlb_request_submit_prompt_logprobs
 #pragma weak llmlb_request_poll_prompt_logprobs
 #pragma weak llmlb_request_cached_tokens
+#pragma weak llmlb_request_submit_choices
 #include "anthropic.hpp"
 #include "checkpoint.hpp"
 #include "download.hpp"
@@ -237,8 +238,25 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
     send_err(404, "The model '" + jm->str() + "' does not exist", "invalid_request_error");
     return;
   }
-  if (const Json* n = req.get("n"))                         // one choice per request: more would be answered with one, silently
-    if (n->is_number() && n->as_int() != 1) { send_err(400, "n must be 1: this endpoint returns one choice per request", "invalid_request_error"); return; }
+  // OpenAI's n: chat and completions serve 1..128 choices of the prompt (llmlb_request_submit_choices: one prefill, its KV
+  // pages forked into the choices); responses and messages have no n, and more than one would be answered with one, silently
+  uint32_t n_choices = 1;
+  if (const Json* n = req.get("n")) {
+    if (kind == 1 || anthropic) {
+      if (n->is_number() && n->as_int() != 1) { send_err(400, "n must be 1: this endpoint returns one choice per request", "invalid_request_error"); return; }
+    } else if (!n->is_null()) {
+      if (!n->is_number() || n->as_double() != double(n->as_int()) || n->as_int() < 1 || n->as_int() > 128) {
+        send_err(400, "n must be an integer in [1, 128]", "invalid_request_error");
+        return;
+      }
+      n_choices = uint32_t(n->as_int());
+      if (n_choices > 1 && !llmlb_request_submit_choices) {
+        send_err(400, "n > 1 is not supported by the engine library this server runs on: it cannot fork a prompt into several choices",
+                 "invalid_request_error");
+        return;
+      }
+    }
+  }
   // prompt
   std::vector<int32_t> ids;
   const std::string* prompt_str = nullptr;   // completions: the prompt as the client sent it, when it is a string
@@ -415,8 +433,11 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
   if (ids.size() + s.max_tokens > G.max_ctx) s.max_tokens = ids.size() < G.max_ctx ? uint32_t(G.max_ctx - ids.size()) : 0;
 
   const auto t0 = std::chrono::steady_clock::now();
-  uint64_t rid = 0;
+  std::vector<uint64_t> rids(n_choices);
+  uint64_t& rid = rids[0];
   int rc = !s.max_tokens ? LLMLB_E_INVALID_ARG
+           : n_choices > 1 ? llmlb_request_submit_choices(G.eng, ids.data(), uint32_t(ids.size()), &s, penalized ? &pen : nullptr,
+                                                          lp_on ? int32_t(lp_top) : -1, lp_prompt ? 1u : 0u, n_choices, rids.data())
            : lp_prompt    ? llmlb_request_submit_prompt_logprobs(G.eng, ids.data(), uint32_t(ids.size()), &s, penalized ? &pen : nullptr, lp_top, &rid)
            : lp_on        ? llmlb_request_submit_logprobs(G.eng, ids.data(), uint32_t(ids.size()), &s, penalized ? &pen : nullptr, lp_top, &rid)
            : penalized    ? llmlb_request_submit_penalized(G.eng, ids.data(), uint32_t(ids.size()), &s, &pen, &rid)
@@ -435,7 +456,11 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
   // every exit path below gives the endpoint's active slot back: a path that forgets to complete
   // the lease finishes it as Error when the lease goes out of scope (balancer/lease.rs:71-100)
   RequestLease lease;
-  if (!G.lm.begin_request_lease(ep, &lease)) { llmlb_request_cancel(G.eng, rid); llmlb_request_release(G.eng, rid); send_err(502, "endpoint disappeared", "endpoint_request_error"); return; }
+  if (!G.lm.begin_request_lease(ep, &lease)) {
+    for (uint64_t r : rids) { llmlb_request_cancel(G.eng, r); llmlb_request_release(G.eng, r); }
+    send_err(502, "endpoint disappeared", "endpoint_request_error");
+    return;
+  }
   const uint64_t n = G.seq.fetch_add(1);
   const std::string id = std::string(kind == 0 ? "chatcmpl-" : kind == 1 ? "resp_" : "cmpl-") + std::to_string(n);
   const int64_t created = int64_t(std::chrono::duration_cast<std::chrono::seconds>(std::chrono::system_clock::now().time_since_epoch()).count());
@@ -451,12 +476,11 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
   };
   if (stream) {
     ok = send_all(fd, "HTTP/1.1 200 OK\r\nContent-Type: text/event-stream\r\nCache-Control: no-cache\r\nTransfer-Encoding: chunked\r\n\r\n");
-    if (kind == 0) ok = ok && send_sse(sse_event(chat_chunk(id, jm->str(), created, &role, nullptr, nullptr)));
+    for (uint32_t c = 0; kind == 0 && c < n_choices; ++c)   // the role delta of every choice first
+      ok = ok && send_sse(sse_event(chat_chunk(id, jm->str(), created, &role, nullptr, nullptr, nullptr, c)));
     if (kind == 1) ok = ok && send_chunk(fd, sse_event(responses_event_created(id, jm->str())) + sse_event(responses_event_item_added()) + sse_event(responses_event_part_added()));
   }
-  std::string text;
-  BpeTokenizer::Stream detok;
-  uint32_t prompt_tokens = uint32_t(ids.size()), completion_tokens = 0, finish = LLMLB_FINISH_NONE;
+  uint32_t prompt_tokens = uint32_t(ids.size());
   auto code_points = [](const std::string& t) { uint32_t n = 0; for (unsigned char c : t) n += (c & 0xC0) != 0x80; return n; };
   // echo: the choice's text starts with the prompt text — the client's string, or the ids through the streaming detokenizer
   // (special tokens skipped, as for generated text); prompt_offs[i] = the code points of that text before prompt token i.
@@ -489,11 +513,24 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
     }
     if (G.tok) prompt_text += BpeTokenizer::flush(&pd);
   }
-  bool prompt_sent = !echo;            // the prompt text (and its entries) went out: stream chunk / head of lp_all
-  // logprobs: every generated token fed to the text path is listed, except the stop ids (their text is skipped)
-  std::vector<LogprobEntry> lp_all;    // the whole list (response body)
-  size_t lp_sent = 0;                  // entries of lp_all already streamed
-  uint32_t text_cps = echo ? code_points(prompt_text) : 0;   // code points of the echoed prompt and `text`
+  // the state of one choice (OpenAI's n; one request id each)
+  struct Choice {
+    uint64_t rid = 0;
+    std::string text;
+    BpeTokenizer::Stream detok;
+    StopMatcher stopper;
+    bool prompt_sent;                    // the prompt text (and its entries) went out: stream chunk / head of lp_all
+    // logprobs: every generated token fed to the text path is listed, except the stop ids (their text is skipped)
+    std::vector<LogprobEntry> lp_all;    // the whole list (response body)
+    size_t lp_sent = 0;                  // entries of lp_all already streamed
+    uint32_t text_cps;                   // code points of the echoed prompt and `text`
+    uint32_t completion_tokens = 0, finish = LLMLB_FINISH_NONE;
+  };
+  std::vector<Choice> chs;
+  for (uint32_t c = 0; c < n_choices; ++c)
+    chs.push_back(Choice{rids[c], std::string(), BpeTokenizer::Stream(), StopMatcher(stop_strings), !echo, {}, 0,
+                         echo ? code_points(prompt_text) : 0});
+  auto cancel_all = [&] { for (auto& ch : chs) llmlb_request_cancel(G.eng, ch.rid); };
   auto lp_token = [&](int32_t id, float v) {
     LogprobToken t;
     t.bytes = G.tok ? G.tok->token_bytes(id) : byte_detokenize(id);
@@ -502,94 +539,118 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
     return t;
   };
   auto lp_json = [&](const std::vector<LogprobEntry>& e) { return kind == 0 ? chat_logprobs(e) : completion_logprobs(e); };
-  while (finish == LLMLB_FINISH_NONE) {
-    llmlb_token_event ev[64];
-    llmlb_token_logprobs lpr[64];
-    uint32_t got = 0;
-    rc = lp_on ? llmlb_request_poll_logprobs(G.eng, rid, ev, lpr, 64, &got, 100) : llmlb_request_poll(G.eng, rid, ev, 64, &got, 100);
-    if (rc != LLMLB_OK && rc != LLMLB_E_TIMEOUT) { finish = LLMLB_FINISH_ERROR; break; }
-    // a client that went away stops the generation, streamed or not — the reference's handler future is dropped with the
-    // connection and its upstream request with it; a buffered response would otherwise run to its last token for nobody
-    if (!client_gone && peer_closed(fd)) { ok = false; client_gone = true; llmlb_request_cancel(G.eng, rid); }
+  bool idle = true;   // n > 1: the last round over the choices brought no event
+  for (;;) {
     std::string out;
-    if (!prompt_sent && got) {   // the first event: every prompt record is queued before it
-      prompt_sent = true;
-      if (lp_prompt) {
-        std::vector<llmlb_token_logprobs> recs;
-        for (uint32_t n_rec = 64; n_rec == 64;) {
-          llmlb_token_logprobs buf[64];
-          n_rec = 0;
-          if (llmlb_request_poll_prompt_logprobs(G.eng, rid, buf, 64, &n_rec) != LLMLB_OK) break;
-          recs.insert(recs.end(), buf, buf + n_rec);
+    bool any = false, got_any = false;
+    for (uint32_t c = 0; c < n_choices; ++c) {
+      Choice& ch = chs[c];
+      if (ch.finish != LLMLB_FINISH_NONE) continue;
+      const bool first = !any;
+      any = true;
+      llmlb_token_event ev[64];
+      llmlb_token_logprobs lpr[64];
+      uint32_t got = 0;
+      // one choice: wait up to 100 ms for events; several: wait on the first unfinished one only after an idle round
+      const int wait = n_choices == 1 ? 100 : first && idle ? 20 : 0;
+      rc = lp_on ? llmlb_request_poll_logprobs(G.eng, ch.rid, ev, lpr, 64, &got, wait) : llmlb_request_poll(G.eng, ch.rid, ev, 64, &got, wait);
+      if (rc != LLMLB_OK && rc != LLMLB_E_TIMEOUT) { ch.finish = LLMLB_FINISH_ERROR; continue; }
+      got_any |= got > 0;
+      // a client that went away stops the generation, streamed or not — the reference's handler future is dropped with the
+      // connection and its upstream request with it; a buffered response would otherwise run to its last token for nobody
+      if (!client_gone && peer_closed(fd)) { ok = false; client_gone = true; cancel_all(); }
+      if (!ch.prompt_sent && got) {   // the first event: every prompt record is queued before it
+        ch.prompt_sent = true;
+        if (lp_prompt) {
+          std::vector<llmlb_token_logprobs> recs;
+          for (uint32_t n_rec = 64; n_rec == 64;) {
+            llmlb_token_logprobs buf[64];
+            n_rec = 0;
+            if (llmlb_request_poll_prompt_logprobs(G.eng, ch.rid, buf, 64, &n_rec) != LLMLB_OK) break;
+            recs.insert(recs.end(), buf, buf + n_rec);
+          }
+          for (size_t k = 0; k < ids.size(); ++k) {
+            LogprobEntry e;
+            e.scored = k > 0 && k - 1 < recs.size();   // the first token has no record; one cut short by a cancel neither
+            e.tok = lp_token(ids[k], e.scored ? recs[k - 1].logprob : 0.f);
+            if (e.scored)
+              for (uint32_t j = 0; j < recs[k - 1].n_top && j < LLMLB_MAX_TOP_LOGPROBS; ++j) e.top.push_back(lp_token(recs[k - 1].top_ids[j], recs[k - 1].top_logprobs[j]));
+            e.text_offset = prompt_offs[k];
+            ch.lp_all.push_back(std::move(e));
+          }
         }
-        for (size_t k = 0; k < ids.size(); ++k) {
-          LogprobEntry e;
-          e.scored = k > 0 && k - 1 < recs.size();   // the first token has no record; one cut short by a cancel neither
-          e.tok = lp_token(ids[k], e.scored ? recs[k - 1].logprob : 0.f);
-          if (e.scored)
-            for (uint32_t j = 0; j < recs[k - 1].n_top && j < LLMLB_MAX_TOP_LOGPROBS; ++j) e.top.push_back(lp_token(recs[k - 1].top_ids[j], recs[k - 1].top_logprobs[j]));
-          e.text_offset = prompt_offs[k];
-          lp_all.push_back(std::move(e));
+        if (stream) {
+          ch.lp_sent = ch.lp_all.size();
+          const Json lj = lp_on ? lp_json(ch.lp_all) : Json();
+          out += sse_event(completion_chunk(id, jm->str(), created, &prompt_text, nullptr, lp_on ? &lj : nullptr, c));
         }
       }
-      if (stream) {
-        lp_sent = lp_all.size();
-        const Json lj = lp_on ? lp_json(lp_all) : Json();
-        out += sse_event(completion_chunk(id, jm->str(), created, &prompt_text, nullptr, lp_on ? &lj : nullptr));
+      for (uint32_t i = 0; i < got; ++i) {
+        if (ev[i].token_id >= 0) {
+          // with a tokenizer a delta only carries complete UTF-8 (a character split over tokens waits)
+          const std::string raw_piece = G.tok ? G.tok->decode_next(&ch.detok, ev[i].token_id, /*skip_special=*/true)
+                                              : byte_detokenize(ev[i].token_id);
+          // a stop string may span tokens: text that could still become one is held back
+          const std::string piece = ch.stopper.feed(raw_piece);
+          if (lp_on && !(!s.ignore_eos && std::find(G.stop_ids.begin(), G.stop_ids.end(), ev[i].token_id) != G.stop_ids.end())) {
+            LogprobEntry e;
+            e.tok = lp_token(ev[i].token_id, lpr[i].logprob);
+            for (uint32_t j = 0; j < lpr[i].n_top && j < LLMLB_MAX_TOP_LOGPROBS; ++j) e.top.push_back(lp_token(lpr[i].top_ids[j], lpr[i].top_logprobs[j]));
+            e.text_offset = ch.text_cps;
+            ch.lp_all.push_back(std::move(e));
+          }
+          ch.text += piece;
+          ch.text_cps += code_points(piece);
+          if (stream && lp_on && (!piece.empty() || ch.lp_sent < ch.lp_all.size())) {
+            // held-back text (a split character, a possible stop prefix) still sends its entries, with empty text
+            const std::vector<LogprobEntry> fresh(ch.lp_all.begin() + ch.lp_sent, ch.lp_all.end());
+            ch.lp_sent = ch.lp_all.size();
+            const Json lj = lp_json(fresh);
+            out += kind == 2 ? sse_event(completion_chunk(id, jm->str(), created, &piece, nullptr, &lj, c))
+                             : sse_event(chat_chunk(id, jm->str(), created, nullptr, &piece, nullptr, &lj, c));
+          } else if (stream && !piece.empty()) out += kind == 1 ? sse_event(responses_event_delta(piece))
+                                       : kind == 2 ? sse_event(completion_chunk(id, jm->str(), created, &piece, nullptr, nullptr, c))
+                                       : sse_event(chat_chunk(id, jm->str(), created, nullptr, &piece, nullptr, nullptr, c));
+        }
+        prompt_tokens = ev[i].prompt_tokens; ch.completion_tokens = ev[i].completion_tokens;
+        if (ev[i].finish_reason) ch.finish = ev[i].finish_reason;
+        if (ch.stopper.hit()) {   // the text ends before the stop string: stop generating this choice, report "stop"
+          llmlb_request_cancel(G.eng, ch.rid);
+          ch.finish = LLMLB_FINISH_STOP;
+          break;
+        }
       }
     }
-    for (uint32_t i = 0; i < got; ++i) {
-      if (ev[i].token_id >= 0) {
-        // with a tokenizer a delta only carries complete UTF-8 (a character split over tokens waits)
-        const std::string raw_piece = G.tok ? G.tok->decode_next(&detok, ev[i].token_id, /*skip_special=*/true)
-                                            : byte_detokenize(ev[i].token_id);
-        // a stop string may span tokens: text that could still become one is held back
-        const std::string piece = stopper.feed(raw_piece);
-        if (lp_on && !(!s.ignore_eos && std::find(G.stop_ids.begin(), G.stop_ids.end(), ev[i].token_id) != G.stop_ids.end())) {
-          LogprobEntry e;
-          e.tok = lp_token(ev[i].token_id, lpr[i].logprob);
-          for (uint32_t j = 0; j < lpr[i].n_top && j < LLMLB_MAX_TOP_LOGPROBS; ++j) e.top.push_back(lp_token(lpr[i].top_ids[j], lpr[i].top_logprobs[j]));
-          e.text_offset = text_cps;
-          lp_all.push_back(std::move(e));
-        }
-        text += piece;
-        text_cps += code_points(piece);
-        if (stream && lp_on && (!piece.empty() || lp_sent < lp_all.size())) {
-          // held-back text (a split character, a possible stop prefix) still sends its entries, with empty text
-          const std::vector<LogprobEntry> fresh(lp_all.begin() + lp_sent, lp_all.end());
-          lp_sent = lp_all.size();
-          const Json lj = lp_json(fresh);
-          out += kind == 2 ? sse_event(completion_chunk(id, jm->str(), created, &piece, nullptr, &lj))
-                           : sse_event(chat_chunk(id, jm->str(), created, nullptr, &piece, nullptr, &lj));
-        } else if (stream && !piece.empty()) out += kind == 1 ? sse_event(responses_event_delta(piece))
-                                     : kind == 2 ? sse_event(completion_chunk(id, jm->str(), created, &piece, nullptr))
-                                     : sse_event(chat_chunk(id, jm->str(), created, nullptr, &piece, nullptr));
-      }
-      prompt_tokens = ev[i].prompt_tokens; completion_tokens = ev[i].completion_tokens;
-      if (ev[i].finish_reason) finish = ev[i].finish_reason;
-      if (stopper.hit()) {   // the text ends before the stop string: stop generating, report "stop"
-        llmlb_request_cancel(G.eng, rid);
-        finish = LLMLB_FINISH_STOP;
-        break;
-      }
-    }
-    if (stream && !out.empty() && ok && !send_sse(out)) { ok = false; client_gone = true; llmlb_request_cancel(G.eng, rid); }
+    if (!any) break;
+    idle = !got_any;
+    if (stream && !out.empty() && ok && !send_sse(out)) { ok = false; client_gone = true; cancel_all(); }
   }
-  if (!stopper.hit()) {  // text held back as a possible stop prefix, and a character cut by the end of generation
-    std::string rest = stopper.feed(G.tok ? BpeTokenizer::flush(&detok) : std::string());
-    if (!stopper.hit()) rest += stopper.flush();
+  uint32_t completion_tokens = 0;   // usage: the prompt counts once, the completions of every choice add up
+  for (uint32_t c = 0; c < n_choices; ++c) {
+    Choice& ch = chs[c];
+    completion_tokens += ch.completion_tokens;
+    if (ch.stopper.hit()) continue;
+    // text held back as a possible stop prefix, and a character cut by the end of generation
+    std::string rest = ch.stopper.feed(G.tok ? BpeTokenizer::flush(&ch.detok) : std::string());
+    if (!ch.stopper.hit()) rest += ch.stopper.flush();
     if (!rest.empty()) {
-      text += rest;
+      ch.text += rest;
       if (stream && ok) send_sse(kind == 1 ? sse_event(responses_event_delta(rest))
-                                 : kind == 2 ? sse_event(completion_chunk(id, jm->str(), created, &rest, nullptr))
-                                 : sse_event(chat_chunk(id, jm->str(), created, nullptr, &rest, nullptr)));
+                                 : kind == 2 ? sse_event(completion_chunk(id, jm->str(), created, &rest, nullptr, nullptr, c))
+                                 : sse_event(chat_chunk(id, jm->str(), created, nullptr, &rest, nullptr, nullptr, c)));
     }
   }
-  // OpenAI's usage.prompt_tokens_details.cached_tokens (input_tokens_details on responses); /v1/messages keeps its shapes
+  // OpenAI's usage.prompt_tokens_details.cached_tokens (input_tokens_details on responses); /v1/messages keeps its shapes.
+  // Every choice of a group reports the group's.
   uint32_t cached = 0;
   const uint32_t* cp = G.prefix_cache && !anthropic && llmlb_request_cached_tokens(G.eng, rid, &cached) == LLMLB_OK ? &cached : nullptr;
-  llmlb_request_release(G.eng, rid);
+  for (auto& ch : chs) llmlb_request_release(G.eng, ch.rid);
   const uint64_t ms = uint64_t(std::chrono::duration_cast<std::chrono::milliseconds>(std::chrono::steady_clock::now() - t0).count());
+  // the request fails if a choice failed; a choice that ended otherwise than by stop or length decides how
+  uint32_t finish = LLMLB_FINISH_STOP;
+  for (auto& ch : chs)
+    if (ch.finish != LLMLB_FINISH_STOP && ch.finish != LLMLB_FINISH_LENGTH) { finish = ch.finish; break; }
+  if (finish == LLMLB_FINISH_STOP) finish = chs[0].finish;
   // streaming drop still counts as success when tokens flowed (openai.rs:2556-2648)
   const bool success = finish == LLMLB_FINISH_STOP || finish == LLMLB_FINISH_LENGTH || (client_gone && completion_tokens > 0);
   {
@@ -597,7 +658,8 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
     lease.complete_with_tokens(success ? RequestOutcome::Success : RequestOutcome::Error, ms, &tu);
   }
   if (success && completion_tokens) G.lm.update_tps(ep, pm.base, api, completion_tokens, std::max<uint64_t>(1, ms));   // `.as_millis().max(1)`: openai.rs:1241-1245, proxy.rs:157
-  const char* fr = finish == LLMLB_FINISH_STOP ? "stop" : "length";
+  auto fr_of = [](uint32_t f) { return f == LLMLB_FINISH_STOP ? "stop" : "length"; };
+  const char* fr = fr_of(chs[0].finish);
   // failures map like the gateway maps an upstream's (openai.rs:862-882, openai_util.rs:86-134)
   const bool failed = finish != LLMLB_FINISH_STOP && finish != LLMLB_FINISH_LENGTH && !(client_gone && completion_tokens > 0);
   ClientError fe = classify_upstream_request_error(UpstreamFailure::Other, 0);                 // the engine failed the request
@@ -622,12 +684,12 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
     }
     std::string tail;
     if (kind == 0) {
-      tail += sse_event(chat_chunk(id, jm->str(), created, nullptr, nullptr, fr));
+      for (uint32_t c = 0; c < n_choices; ++c) tail += sse_event(chat_chunk(id, jm->str(), created, nullptr, nullptr, fr_of(chs[c].finish), nullptr, c));
       if (include_usage) tail += sse_event(chat_usage_chunk(id, jm->str(), created, prompt_tokens, completion_tokens, cp));
     } else if (kind == 1) {
-      tail += sse_event(responses_event_text_done(text)) + sse_event(responses_event_done(id, prompt_tokens, completion_tokens, cp));
-    } else {   // legacy completions: text_completion chunks, a finish chunk, optional usage
-      tail += sse_event(completion_chunk(id, jm->str(), created, nullptr, fr));
+      tail += sse_event(responses_event_text_done(chs[0].text)) + sse_event(responses_event_done(id, prompt_tokens, completion_tokens, cp));
+    } else {   // legacy completions: text_completion chunks, a finish chunk per choice, optional usage
+      for (uint32_t c = 0; c < n_choices; ++c) tail += sse_event(completion_chunk(id, jm->str(), created, nullptr, fr_of(chs[c].finish), nullptr, c));
       if (include_usage) tail += sse_event(completion_usage_chunk(id, jm->str(), created, prompt_tokens, completion_tokens, cp));
     }
     tail += sse_done();
@@ -641,14 +703,19 @@ static void handle_generate(int fd, const Request& rq, int kind, const Json* pre
     }
     send_all(fd, "0\r\n\r\n");
   } else if (anthropic) {
-    const Json chat = chat_completion_body(id, jm->str(), created, text, fr, prompt_tokens, completion_tokens);
+    const Json chat = chat_completion_body(id, jm->str(), created, chs[0].text, fr, prompt_tokens, completion_tokens);
     send_json(fd, 200, openai_to_anthropic_message_response(chat, jm->str(), prompt_tokens, completion_tokens, "msg_" + std::to_string(n)).dump());
+  } else if (kind == 1) {
+    send_json(fd, 200, responses_body(id, jm->str(), created, chs[0].text, prompt_tokens, completion_tokens, "completed", cp).dump());
   } else {
-    const Json lj = lp_on ? lp_json(lp_all) : Json();
-    const Json* lpp = lp_on ? &lj : nullptr;
-    Json body = kind == 0 ? chat_completion_body(id, jm->str(), created, text, fr, prompt_tokens, completion_tokens, lpp, cp)
-              : kind == 1 ? responses_body(id, jm->str(), created, text, prompt_tokens, completion_tokens, "completed", cp)
-                          : completion_body(id, jm->str(), created, prompt_text + text, fr, prompt_tokens, completion_tokens, lpp, cp);
+    std::vector<Json> ljs(n_choices);   // every choice's "logprobs" value, kept alive for `outs`
+    std::vector<ChoiceOut> outs(n_choices);
+    for (uint32_t c = 0; c < n_choices; ++c) {
+      if (lp_on) ljs[c] = lp_json(chs[c].lp_all);
+      outs[c] = ChoiceOut{kind == 2 ? prompt_text + chs[c].text : chs[c].text, fr_of(chs[c].finish), lp_on ? &ljs[c] : nullptr};
+    }
+    const Json body = kind == 0 ? chat_completion_body(id, jm->str(), created, outs, prompt_tokens, completion_tokens, cp)
+                                : completion_body(id, jm->str(), created, outs, prompt_tokens, completion_tokens, cp);
     send_json(fd, 200, body.dump());
   }
 }
