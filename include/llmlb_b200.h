@@ -393,6 +393,15 @@ int llmlb_op_decode_attention(const void* qkv_bf16, void* k_pages, void* v_pages
                               void* out_bf16, uint32_t n_heads, uint32_t n_kv_heads,
                               const float* rope_table, uint32_t n_splits, uint32_t ws_seqs,
                               void* workspace, void* stream);
+/* The same decode attention as the engine launches it, for kernel tests: pdl != 0 makes it a programmatic dependent
+ * launch (the engine's layers >= 1 at up to 4 sequences), whose prologue prefetches K/V while the kernel before it
+ * (the QKV projection) is still running and reads qkv only after that kernel has completed. */
+int llmlb_debug_decode_attention(const void* qkv_bf16, void* k_pages, void* v_pages,
+                                 const int32_t* block_tables, uint32_t bt_stride,
+                                 const int32_t* bt_rows, const int32_t* seq_lens, uint32_t n_seqs,
+                                 void* out_bf16, uint32_t n_heads, uint32_t n_kv_heads,
+                                 const float* rope_table, uint32_t n_splits, uint32_t ws_seqs,
+                                 void* workspace, uint32_t pdl, void* stream);
 /* a2.12 sampling: arg-max when temperature==0 else temperature/top-k/top-p with a counter RNG.
  * params: per-row {temperature, top_p} floats, {top_k} ints, {seed, step} u64. */
 int llmlb_op_sample(const float* logits, uint32_t n_rows, uint32_t vocab, const float* temperature,

@@ -955,3 +955,14 @@ extern "C" int llmlb_op_decode_attention(const void* qkv, void* k_pages, void* v
   return decode_attention_launch(qkv, k_pages, v_pages, block_tables, bt_stride, bt_rows, seq_lens, n_seqs, out,
                                  n_heads, n_kv, rope_table, n_splits, false, (cudaStream_t)stream);
 }
+
+// The same launch as the engine's attention_block makes it: pdl != 0 is a programmatic dependent launch (layers >= 1)
+extern "C" int llmlb_debug_decode_attention(const void* qkv, void* k_pages, void* v_pages,
+                                            const int32_t* block_tables, uint32_t bt_stride,
+                                            const int32_t* bt_rows, const int32_t* seq_lens,
+                                            uint32_t n_seqs, void* out, uint32_t n_heads,
+                                            uint32_t n_kv, const float* rope_table,
+                                            uint32_t n_splits, uint32_t, void*, uint32_t pdl, void* stream) {
+  return decode_attention_launch(qkv, k_pages, v_pages, block_tables, bt_stride, bt_rows, seq_lens, n_seqs, out,
+                                 n_heads, n_kv, rope_table, n_splits, pdl != 0, (cudaStream_t)stream);
+}

@@ -126,6 +126,8 @@ PROTOTYPES = {
     "llmlb_op_decode_attention_ws": (C.c_size_t, [u32, u32, u32]),
     "llmlb_op_decode_attention": (C.c_int, [vp, vp, vp, vp, u32, vp, vp, u32, vp, u32, u32, vp,
                                             u32, u32, vp, vp]),
+    "llmlb_debug_decode_attention": (C.c_int, [vp, vp, vp, vp, u32, vp, vp, u32, vp, u32, u32, vp,
+                                               u32, u32, vp, u32, vp]),
     "llmlb_op_sample": (C.c_int, [vp, u32, u32, vp, vp, vp, vp, vp, vp, vp]),
     "llmlb_op_penalize": (C.c_int, [vp, u32, u32, vp, u64, vp, vp, vp, vp, vp, u32, vp]),
     "llmlb_op_logprobs": (C.c_int, [vp, u32, u32, vp, vp, vp, vp]),

@@ -214,7 +214,8 @@ cudaError_t cudaGraphExecDestroy(cudaGraphExec_t x) { free(x); return cudaSucces
 // (gemv_ks_kernel, whose 9th parameter is TW, the warps of a team) append TW, which sets the kernel's team count.  The
 // residual fold (rmsnorm_parts_kernel / rmsnorm_parts_cluster_kernel) appends n_parts, whether a gain was given (0 / 1)
 // and hidden; rope_append_kernel appends n_heads and n_kv; rmsnorm_kernel and embed_kernel append hidden; sample_kernel
-// appends vocab.
+// appends vocab; both decode attention kernels append n_heads, n_kv and the sequence count (grid z of the cluster kernel,
+// grid y of the tensor-core kernel).
 static void log_launch(const void* fn, dim3 g, dim3 b, size_t smem, dim3 cluster, int pdl, void** args = nullptr) {
   static FILE* f = getenv("FAKE_CUDART_LAUNCH_LOG") ? fopen(getenv("FAKE_CUDART_LAUNCH_LOG"), "a") : nullptr;
   if (!f) return;
@@ -230,6 +231,9 @@ static void log_launch(const void* fn, dim3 g, dim3 b, size_t smem, dim3 cluster
   if (args && strstr(name, "18rope_append_kernel")) fprintf(f, " %u %u", u32(6), u32(7));
   if (args && (strstr(name, "14rmsnorm_kernel") || strstr(name, "12embed_kernel"))) fprintf(f, " %u", u32(3));
   if (args && strstr(name, "13sample_kernel")) fprintf(f, " %u", u32(1));     // (logits, vocab, ...)
+  // (qkv, k_pages, v_pages, block_tables, bt_stride, bt_rows, seq_lens, rope, out, n_heads, n_kv, ...)
+  if (args && strstr(name, "23decode_attention_kernel")) fprintf(f, " %u %u %u", u32(9), u32(10), g.z);
+  if (args && strstr(name, "27decode_attention_mma_kernel")) fprintf(f, " %u %u %u", u32(9), u32(10), g.y);
   fputc('\n', f);
   fflush(f);
 }

@@ -1,11 +1,13 @@
 """The launches of the GPU kernel tests (tests/test_kernels_sm90_gpu.py, tests/test_gemv_sm90_gpu.py,
-tests/test_step_kernels_sm90_gpu.py), made over the fake CUDA runtime with FAKE_CUDART_LAUNCH_LOG set: every GEMM case through
-the entry point it uses there, the wave-tail pair, every decode split, both prefill attention kernels, every GEMV case through
+tests/test_step_kernels_sm90_gpu.py, tests/test_decode_attention_sm90_gpu.py), made over the fake CUDA runtime with
+FAKE_CUDART_LAUNCH_LOG set: every GEMM case through the entry point it uses there, the wave-tail pair, every decode split,
+every decode attention case, the decode layer chain's first two layers, both prefill attention kernels, every GEMV case through
 llmlb_op_gemv, the residual fold, RMSNorm, RoPE / KV-append and embedding cases, and the sampler's vocabularies
 (tests/test_sampling_sm90_gpu.py).  Nothing executes; the log is the launch
 plan of the test cases.  Every section is optional.
 usage: kernel_case_sweep.py <cases.json>   ({"gemm": [[T, n_out, K, epi], ...], "wave_tail": [T, n_out, K, main_rows],
                                              "decode_splits": [...], "max_split": n,
+                                             "decode": [[splits, n_heads, n_kv, batch], ...], "chain": [batch, ...],
                                              "gemv": [[n_out, K, tokens, epi, norm, out_stride], ...],
                                              "fold": [[T, H, n_parts, gain, part_stride], ...], "rmsnorm": [[T, H], ...],
                                              "rope": [[T, n_heads, n_kv], ...], "embed": [[T, H, vocab], ...],
@@ -17,6 +19,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 from llmlb_b200 import ffi  # noqa: E402
 
 L = ffi.lib()
@@ -57,6 +60,22 @@ rope, ws = dmalloc(1 << 20), dmalloc(256)
 for sp in cases.get("decode_splits", []):
     mark("decode %d" % sp)
     ffi.check(L.llmlb_op_decode_attention(x, w, w, out, 66, out, out, 5, out, 32, 8, rope, sp, 5, ws, None))
+for sp, nh, nkv, B in cases.get("decode", []):
+    mark("decode case %d %d %d %d" % (sp, nh, nkv, B))
+    ffi.check(L.llmlb_debug_decode_attention(x, w, w, out, 66, out, out, B, out, nh, nkv, rope, sp, B, ws, 0, None))
+
+
+def chain_arg(name, l):
+    """The decode layer chain's arguments: weights and pools in w, activations in x, block tables and lengths in out."""
+    if name == "bt_stride":
+        return 66
+    return {"x": x, "qkv": x, "attn": x, "h": x, "bt": out, "rows": out, "seq_lens": out, "rope": rope, "ws": ws}.get(name, w)
+
+
+for B in cases.get("chain", []):
+    mark("chain B=%d" % B)
+    import test_gemv_sm90_gpu as GV
+    GV.chain_launches(L, B, 2, chain_arg, lambda: None)
 if "decode_splits" in cases:
     mark("prefill")
     ffi.check(L.llmlb_op_prefill_attention_tc(x, 300, w, w, 80, out, 66, out, 3, out, 32, 8, None))

@@ -3,7 +3,7 @@ log holds the engine's LAUNCH PLAN — kernel, grid, block, shared memory, clust
 every decode batch width 1..128 of a model geometry / tensor-parallel degree.  Two layers only: launch shapes do not depend
 on the depth.  All `tp` ranks live in this one process (the fake runtime's IPC handles work within a process too) and run one
 after the other: nothing executes, so nobody waits for a peer.
-usage: launch_plan_sweep.py 8b|mid|70b <tp> [max_width]
+usage: launch_plan_sweep.py 8b|mid|70b|tiny <tp> [max_width]
   max_width: only prefill widths and decode batches up to it (the long-context batches too), and no 131072-token context —
   enough to see every decode GEMV launch (those run at 1..4 rows only) without the cost of the whole sweep."""
 import os
@@ -14,7 +14,7 @@ sys.path.insert(0, ROOT)
 from llmlb_b200 import ffi  # noqa: E402
 
 LOG = os.environ["FAKE_CUDART_LAUNCH_LOG"]
-MODELS = {"8b": ffi.LLAMA3_8B, "mid": ffi.LLAMA_MID, "70b": ffi.LLAMA3_70B}
+MODELS = {"8b": ffi.LLAMA3_8B, "mid": ffi.LLAMA_MID, "70b": ffi.LLAMA3_70B, "tiny": ffi.LLAMA_TINY}
 
 
 def mark(s):

@@ -1,4 +1,4 @@
-"""Random arguments into every kernel-level entry point (llmlb_op_*, and llmlb_debug_rmsnorm_parts) on the fake CUDA runtime: pointers are valid device
+"""Random arguments into every kernel-level entry point (llmlb_op_*, llmlb_debug_rmsnorm_parts and llmlb_debug_decode_attention) on the fake CUDA runtime: pointers are valid device
 allocations or NULL, integers come from {0, 1, small, odd, the model's, huge}.  Nothing executes; what is tested is the HOST
 side of each entry point: every call returns (OK or a negative error code) — no crash, no division by zero, no launch the
 fake runtime refuses for its shape (block > 1024 threads, shared memory without opt-in, broken cluster).
@@ -43,7 +43,7 @@ def f():
 calls = crashes = 0
 hist = {}
 for _ in range(int(sys.argv[1])):
-    op = rs.randrange(13)
+    op = rs.randrange(14)
     if op == 0:
         rc = L.llmlb_op_embed(ptr(), ptr(), ptr(), u(), u(), u(), None)
     elif op == 1:
@@ -69,6 +69,9 @@ for _ in range(int(sys.argv[1])):
         rc = L.llmlb_op_synth_bf16(ptr(), u(), u(), u(), u(), u(), u(), rs.randrange(40), f(), None)
     elif op == 11:
         rc = L.llmlb_op_allreduce(None, ptr(), u(), None)
+    elif op == 13:
+        rc = L.llmlb_debug_decode_attention(ptr(), ptr(), ptr(), ptr(), u(), ptr(), ptr(), u(), ptr(), u(), u(), ptr(), u(), u(), ptr(),
+                                            rs.choice([0, 1, u()]), None)
     else:
         rc = L.llmlb_debug_rmsnorm_parts(ptr(), ptr(), rs.choice([0, 1, 2, 4, 8, 16, 17, u()]), rs.choice([0, u(), u() * u()]),
                                          ptr(), ptr(), u(), u(), f(), None)

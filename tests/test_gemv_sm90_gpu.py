@@ -19,8 +19,8 @@ Two kinds of input, as for the GEMMs (tests/test_kernels_sm90_gpu.py, whose help
   * random data against fp64, with zeroed W rows, one W row x 2^10, a zeroed token and per-token scales 8x apart (a token
     that borrows another's RMS scale is off by 8x).  Elementwise bounds derived from |y| |W|^T.
 Every output lands inside a NaN-sentinel guard band (rows before and after, out_stride = n_cols + PAD) that must come back
-unchanged.  A chain test runs four Llama-3-8B decode layers back to back and checks them bit for bit against the same
-launches with a synchronize after each and against a CUDA-graph replay.
+unchanged.  A chain test runs four Llama-3-8B decode layers, decode attention included, back to back and checks them bit for
+bit against the same launches with a synchronize after each and against a CUDA-graph replay.
 
 GEMV_CASES is plain data: tests/test_kernel_coverage_cpu.py runs it through llmlb_op_gemv over the fake CUDA runtime and
 checks that it launches every GEMV class the engine launches at Llama-3-8B, LLAMA_MID and Llama-3-70B shapes.
@@ -31,6 +31,7 @@ import pytest
 
 from test_kernels_sm90_gpu import (BF16_U, EPI_RESID_F32, EPI_SILU_MUL, EPI_STORE_BF16, EPI_STORE_F32, _Out, _report,
                                    bits_equal, gemm_acc_bound, probe_weights, silu_eval_rel, silu_mul_ref)
+from test_step_kernels_sm90_gpu import rope_table  # noqa: F401 (fixture)
 
 # ---------------------------------------------------------------------------------------------------------------- cases --
 ALL = (EPI_STORE_BF16, EPI_RESID_F32, EPI_SILU_MUL, EPI_STORE_F32)
@@ -353,6 +354,9 @@ def test_gemv_random_data_within_fp64_bound(L, N, K, B, epi, norm):
 # ------------------------------------------------------------------------------------------------ one decode layer --
 CHAIN_LAYERS = 4
 CHAIN_H, CHAIN_QKV, CHAIN_FFN = 4096, 6144, 14336     # Llama-3-8B
+CHAIN_HEADS, CHAIN_KV = 32, 8
+CHAIN_BATCHES = (1, 2, 3, 4)                          # decode_splits: 16 at B = 1, 2, 11 (a cluster of 8) at 3, 9 at 4
+CHAIN_CTX = (300, 4097)                               # each layer's context per sequence (with the new token): in this range
 
 
 @pytest.fixture(scope="module")
@@ -368,71 +372,133 @@ def chain_weights():
             for _ in range(CHAIN_LAYERS)]
 
 
-def _chain(L, lw, x, attn, qkv, h, B, depth, sync_each=False, snaps=None):
-    """The decode layer's GEMVs as forward_tokens launches them at B <= 4, attention replaced by the fixed input `attn`:
-    QKV (NORM, bf16 out), O (residual into x), gate/up (NORM, SiLU), down (residual into x)."""
-    import torch
-    from gpu_util import ok, p, stream_ptr
+def chain_launches(L, B, depth, arg, stream, after=None):
+    """The decode layer as forward_tokens launches it at B <= 4 sequences and tp = 1, layers 0..depth-1: QKV (NORM, bf16
+    out), decode attention (a plain launch at layer 0, a programmatic dependent from layer 1 on, with the engine's split for
+    B), O (residual into x), gate/up (NORM, SiLU), down (residual into x).  arg(name, l) is layer l's device pointer of
+    wqkv, wo, wgu, wdown, g_attn, g_ffn, x, qkv, attn, h, kp, vp, bt, rows, seq_lens, rope, ws, or its bt_stride;
+    after(launch index in the layer, l) runs after each launch."""
+    from llmlb_b200 import ffi
+    from test_decode_attention_sm90_gpu import decode_splits
     H, Q, F = CHAIN_H, CHAIN_QKV, CHAIN_FFN
+    splits = decode_splits(B, CHAIN_HEADS)
 
-    def go(w, xin, gain, out, n_out, k, epi, stride):
-        ok(L.llmlb_op_gemv(p(w), p(xin), p(gain), 1e-5, p(out), B, n_out, k, epi, stride, stream_ptr()))
-        if sync_each:
-            torch.cuda.current_stream().synchronize()
+    def gemv(l, w, xin, gain, out, n_out, k, epi, stride):
+        ffi.check(L.llmlb_op_gemv(arg(w, l), arg(xin, l), arg(gain, l) if gain else None, 1e-5, arg(out, l), B, n_out, k, epi, stride,
+                                  stream()))
+
+    def attention(l):
+        ffi.check(L.llmlb_debug_decode_attention(arg("qkv", l), arg("kp", l), arg("vp", l), arg("bt", l), arg("bt_stride", l),
+                                                 arg("rows", l), arg("seq_lens", l), B, arg("attn", l), CHAIN_HEADS, CHAIN_KV,
+                                                 arg("rope", l), splits, B, arg("ws", l), int(l > 0), stream()))
     for l in range(depth):
-        w = lw[l]
-        go(w["wqkv"], x, w["g_attn"], qkv[l], Q, H, EPI_STORE_BF16, Q)
-        go(w["wo"], attn, None, x, H, H, EPI_RESID_F32, H)
-        go(w["wgu"], x, w["g_ffn"], h[l], 2 * F, H, EPI_SILU_MUL, F)
-        go(w["wdown"], h[l], None, x, H, F, EPI_RESID_F32, H)
-        if snaps is not None:
-            snaps.append(x.clone())
+        launches = [lambda: gemv(l, "wqkv", "x", "g_attn", "qkv", Q, H, EPI_STORE_BF16, Q), lambda: attention(l),
+                    lambda: gemv(l, "wo", "attn", None, "x", H, H, EPI_RESID_F32, H),
+                    lambda: gemv(l, "wgu", "x", "g_ffn", "h", 2 * F, H, EPI_SILU_MUL, F),
+                    lambda: gemv(l, "wdown", "h", None, "x", H, F, EPI_RESID_F32, H)]
+        for i, run in enumerate(launches):
+            run()
+            if after:
+                after(i, l)
 
 
-@pytest.mark.parametrize("B", [1, 2, 4])
-def test_decode_layer_chain_is_bit_identical_back_to_back_synchronised_and_graphed(L, chain_weights, B):
-    """Four layers launched back to back on one stream (the K-split kernels as programmatic dependents; at B >= 2 the down
-    projection is the row-owner kernel, launched without PDL, between them) must give exactly what the same launches give
-    with a synchronize after each, and so must a CUDA-graph replay of them — qkv, h and x after every layer."""
+@pytest.mark.parametrize("B", CHAIN_BATCHES)
+def test_decode_layer_chain_is_bit_identical_back_to_back_synchronised_and_graphed(L, chain_weights, rope_table, B):
+    """Four layers, each with its own K/V pool and contexts of 300..4097 tokens, launched back to back on one stream as the
+    engine does (the K-split GEMVs and, from layer 1 on, decode attention as programmatic dependents: attention's prologue
+    prefetches K/V while the QKV GEMV runs and must read qkv only after it; the O GEMV streams its weights while attention
+    runs) must give exactly what the same launches give with a synchronize after each, and so must a CUDA-graph replay of
+    them — qkv, attn, h, the appended K/V of every layer and x after every layer.  Each layer's attention output and
+    pools, from the synchronised run, meet the reference of tests/test_decode_attention_sm90_gpu.py on that layer's own qkv."""
     import torch
-    from gpu_util import sync
+    from gpu_util import p, sync
+    from test_decode_attention_sm90_gpu import Pool, check_launch, decode_splits, rope_rotate
     from test_kernels_sm90_gpu import SENT16
     H, Q, F = CHAIN_H, CHAIN_QKV, CHAIN_FFN
     gen = torch.Generator(device="cuda").manual_seed(B)
     x0 = torch.randn(B, H, generator=gen, device="cuda")
-    attn = torch.randn(B, H, generator=gen, device="cuda").to(torch.bfloat16)
     x = torch.empty_like(x0)
     qkv = [torch.empty(B, Q, dtype=torch.bfloat16, device="cuda") for _ in range(CHAIN_LAYERS)]
+    attn = [torch.empty(B, H, dtype=torch.bfloat16, device="cuda") for _ in range(CHAIN_LAYERS)]
     h = [torch.empty(B, F, dtype=torch.bfloat16, device="cuda") for _ in range(CHAIN_LAYERS)]
+    lens = torch.randint(CHAIN_CTX[0], CHAIN_CTX[1] + 1, (CHAIN_LAYERS, B), generator=torch.Generator().manual_seed(B)).tolist()
+    lens[0][0] = CHAIN_CTX[1]
+    pools, ctx = [], []
+    for l in range(CHAIN_LAYERS):
+        pool = Pool(CHAIN_KV, lens[l], 100 * B + l)
+        ck = [torch.randn(n - 1, CHAIN_KV, 128, generator=gen, device="cuda").to(torch.bfloat16) for n in lens[l]]
+        cv = [torch.randn(n - 1, CHAIN_KV, 128, generator=gen, device="cuda").to(torch.bfloat16) for n in lens[l]]
+        for i in range(B):
+            pool.write(i, 0, ck[i], cv[i])
+        pools.append(pool)
+        ctx.append((ck, cv))
+    pool0 = [(pl.kp.clone(), pl.vp.clone()) for pl in pools]
+    seq_lens = [torch.tensor(n, dtype=torch.int32, device="cuda") for n in lens]
+    ws = torch.zeros(256, dtype=torch.uint8, device="cuda")
+    shared = dict(x=x, rope=rope_table, ws=ws)
+
+    def arg(name, l):
+        if name in chain_weights[l]:
+            return p(chain_weights[l][name])
+        if name in shared:
+            return p(shared[name])
+        if name in ("kp", "vp", "bt", "rows"):
+            return p(getattr(pools[l], name))
+        if name == "bt_stride":
+            return pools[l].bt_stride
+        return p({"qkv": qkv, "attn": attn, "h": h, "seq_lens": seq_lens}[name][l])
+
+    def stream():
+        from gpu_util import stream_ptr
+        return stream_ptr()
 
     def reset():
         x.copy_(x0)
-        for t in qkv + h:
+        for t in qkv + attn + h:
             t.view(torch.int16).fill_(SENT16)
+        for pl, (k0, v0) in zip(pools, pool0):
+            pl.kp.copy_(k0)
+            pl.vp.copy_(v0)
 
     reset()
     snaps = []
-    _chain(L, chain_weights, x, attn, qkv, h, B, CHAIN_LAYERS, sync_each=True, snaps=snaps)
+
+    def after(i, l):
+        torch.cuda.current_stream().synchronize()
+        if i == 4:
+            snaps.append(x.clone())
+    chain_launches(L, B, CHAIN_LAYERS, arg, stream, after)
     sync()
-    want_qkv, want_h = [t.clone() for t in qkv], [t.clone() for t in h]
-    assert all(bool(torch.isfinite(t.float()).all()) for t in want_qkv + want_h + snaps)
+    want = {"qkv": [t.clone() for t in qkv], "attn": [t.clone() for t in attn], "h": [t.clone() for t in h],
+            "kp": [pl.kp.clone() for pl in pools], "vp": [pl.vp.clone() for pl in pools]}
+    assert all(bool(torch.isfinite(t.float()).all()) for t in want["qkv"] + want["attn"] + want["h"] + snaps)
     assert all(bits_equal(snaps[l], snaps[l + 1]) > 0 for l in range(CHAIN_LAYERS - 1))    # every layer moves x
+    splits, ratio = decode_splits(B, CHAIN_HEADS), 0.0
+    for l, pl in enumerate(pools):
+        rot = rope_rotate(L, want["qkv"][l], seq_lens[l] - 1, rope_table, CHAIN_HEADS, CHAIN_KV)
+        sync()
+        ratio = max(ratio, check_launch(L, rope_table, pl, pool0[l][0], pool0[l][1], want["qkv"][l], rot, want["attn"][l], ctx[l][0],
+                                        ctx[l][1], seq_lens[l], CHAIN_HEADS, CHAIN_KV, splits, "layer %d" % l))
+    _report("decode layer chain attention", ratio)
 
     def check(mode, depth):
+        got = {"qkv": qkv, "attn": attn, "h": h, "kp": [pl.kp for pl in pools], "vp": [pl.vp for pl in pools]}
         for l in range(depth):
-            assert bits_equal(qkv[l], want_qkv[l]) == 0, "%s, %d layers: qkv of layer %d differs" % (mode, depth, l)
-            assert bits_equal(h[l], want_h[l]) == 0, "%s, %d layers: h of layer %d differs" % (mode, depth, l)
+            for name in ("qkv", "attn", "h", "kp", "vp"):
+                assert bits_equal(got[name][l], want[name][l]) == 0, "%s, %d layers: %s of layer %d differs" % (mode, depth, name, l)
+        for l in range(depth, CHAIN_LAYERS):
+            assert bits_equal(pools[l].kp, pool0[l][0]) == 0 and bits_equal(pools[l].vp, pool0[l][1]) == 0, (mode, depth, l)
         assert bits_equal(x, snaps[depth - 1]) == 0, "%s: x after layer %d differs" % (mode, depth - 1)
 
     for depth in range(1, CHAIN_LAYERS + 1):
         reset()
-        _chain(L, chain_weights, x, attn, qkv, h, B, depth)
+        chain_launches(L, B, depth, arg, stream)
         sync()
         check("back to back", depth)
     for depth in range(1, CHAIN_LAYERS + 1):     # the eager runs above made every shared-memory opt-in outside capture
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
-            _chain(L, chain_weights, x, attn, qkv, h, B, depth)
+            chain_launches(L, B, depth, arg, stream)
         reset()
         g.replay()
         sync()

@@ -21,6 +21,14 @@ would notice the mistakes they are meant to catch.
     launched by a GPU kernel test case or listed with the test that covers it; and the fold, norm and RoPE checkers reject
     a dropped or reordered part, a gain a quarter off, a missing DSMEM exchange, another token's RMS scale, wrong RoPE
     pairs, positions or sin sign, and K in the neighbouring page slot.
+  * decode attention (tests/test_decode_attention_sm90_gpu.py): DECODE_CASES is decode_splits' classes at their smallest and
+    largest batch, and launches every (cluster size, n_heads, n_kv) class the engine's plans launch — tp = 1 at Llama-3-8B,
+    LLAMA_TINY, LLAMA_MID and Llama-3-70B shapes, the 8B and 70B shards at tp 2, 4 and 8, decode batches 1..128 — at the
+    smallest and the largest batch the engine launches it at; the decode layer chain of tests/test_gemv_sm90_gpu.py makes
+    exactly the engine's launches of a decode step's first two layers at B = 1..4 (kernel, grid, block, cluster, shared
+    memory, PDL); and the decode checkers reject a kernel that rotates with the identity table, at position L, with the sin
+    sign flipped or interleaved pairs, attends over the stale page row instead of the new token, appends k to the next
+    slot or the neighbouring kv head, reads another head group's kv head, or attends with the previous layer's qkv rows.
   * sampler (tests/test_sampling_sm90_gpu.py): its vocabularies cover every vocabulary the engine samples at 8B, MID and
     70B; and its draw checker, applied to a numpy model of the kernel's fp32 orders, rejects the old fallback to the last
     kept index on draws inside the gap between the warp totals and the row scans, a run not carried across rows, a strict
@@ -40,6 +48,7 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
+import test_decode_attention_sm90_gpu as DA  # noqa: E402
 import test_engine_host_logic_cpu as HL  # noqa: E402
 import test_gemv_sm90_gpu as GV  # noqa: E402
 import test_kernels_sm90_gpu as K  # noqa: E402
@@ -63,7 +72,8 @@ FOLD_KERNELS = ("rmsnorm_parts_kernel", "rmsnorm_parts_cluster_kernel")
 
 def classes(log):
     """{context: set of launch classes}: ("gemm_tc_kernel" | "gemm_tc2_kernel", BN, EPI, K-split) for the projections,
-    ("decode", cluster size) for decode attention (1 = the unsplit tensor-core kernel), ("prefill", kernel),
+    ("decode", cluster size, n_heads, n_kv) for decode attention (cluster size 1 = the unsplit tensor-core kernel),
+    ("prefill", kernel),
     ("gemv_ks", B, EPI, NORM, CW, TW) for the K-split GEMV, ("gemv", B, EPI, NORM) for the row-owner GEMV,
     ("fold", kernel, n_parts, gain, H) for the residual fold, ("rope", n_heads, n_kv), ("rmsnorm_kernel", H) and
     ("embed_kernel", H) and ("sample", vocab)."""
@@ -104,9 +114,11 @@ def classes(log):
         if m:
             out[ctx].add(("gemv", int(m.group(1)), int(m.group(2)), m.group(3) == "1"))
         elif "decode_attention_mma_kernel" in p[0]:
-            out[ctx].add(("decode", 1))
+            assert len(p) == 15, line            # n_heads, n_kv, sequences appended
+            out[ctx].add(("decode", 1, int(p[12]), int(p[13])))
         elif "decode_attention_kernel" in p[0]:
-            out[ctx].add(("decode", int(p[8])))
+            assert len(p) == 15, line
+            out[ctx].add(("decode", int(p[8]), int(p[12]), int(p[13])))
         elif "prefill_attention_kernel_tc" in p[0]:
             out[ctx].add(("prefill", "tc"))
         elif "prefill_attention_kernel" in p[0]:
@@ -153,7 +165,7 @@ def test_gpu_cases_launch_every_class_the_engine_launches(built_lib, tmp_path):
         engine |= set().union(*plan.values())
     engine_gemm = {c for c in engine if c[0].startswith("gemm") and c[2] <= 4}
     engine_attn = {c for c in engine if c[0] in ("decode", "prefill")}
-    assert len(engine_gemm) >= 20 and {("decode", s) for s in (1, 2, 4, 8, 16)} <= engine_attn, sorted(engine)
+    assert len(engine_gemm) >= 20 and {("decode", s, 32, 8) for s in (1, 2, 4, 8, 16)} <= engine_attn, sorted(engine)
     missing = sorted((engine_gemm | engine_attn) - tested)
     assert not missing, "the engine launches classes no GPU kernel test runs: %s" % missing
 
@@ -735,6 +747,166 @@ def test_rope_checker_rejects_wrong_pairs_positions_sin_sign_and_slot():
     assert _rope_rejects(pos_shift=-1) > 0
     assert _rope_rejects(sin_sign=-1.0) > 0
     assert _rope_rejects(slot_shift=1) > 0
+
+
+# ---------------------------------------------------------------------------------------------------- decode attention --
+DECODE_PLANS = [("tiny", 1), ("mid", 1), ("8b", 1), ("70b", 1)] + [(m, tp) for m in ("8b", "70b") for tp in (2, 4, 8)]
+DECODE_KERNELS = ("decode_attention_kernel", "decode_attention_mma_kernel")
+
+
+def decode_launches(log):
+    """{(cluster size, n_heads, n_kv, sequences)} of the decode attention launches in a log (1 = the tensor-core kernel)."""
+    out = set()
+    for p in (l.split() for l in open(log) if not l.startswith("###")):
+        name = short_name(p[0])
+        if name in DECODE_KERNELS:
+            assert len(p) == 15, p
+            out.add((int(p[8]) if name == DECODE_KERNELS[0] else 1, int(p[12]), int(p[13]), int(p[14])))
+    return out
+
+
+def launch_lines(log):
+    """{context: [fields of each launch]}, in launch order."""
+    out, ctx = collections.defaultdict(list), "init"
+    for line in open(log):
+        if line.startswith("###"):
+            ctx = line[4:].strip()
+        else:
+            out[ctx].append(line.split())
+    return out
+
+
+def test_decode_cases_are_every_decode_splits_class_at_its_smallest_and_largest_batch():
+    assert DA.DECODE_CASES == DA.derived_cases()
+    assert len({(DA.cluster_size(sp), nh, nkv) for sp, nh, nkv, _ in DA.DECODE_CASES}) == 39
+    # the cluster kernel on narrow shards at wide batches, the tensor-core kernel up to 128 sequences
+    assert (3, 4, 1, 95) in DA.DECODE_CASES and (1, 4, 1, 96) in DA.DECODE_CASES and (1, 64, 8, 128) in DA.DECODE_CASES
+    for B in (1, 4, 9, 128):
+        lens = DA.launch_lens(B)
+        flat = [n for launch in lens for n in launch]
+        assert all(len(launch) == B for launch in lens) and set(flat) == set(DA.LENS) | {DA.LONG} and flat.count(DA.LONG) == 1
+
+
+def test_gpu_decode_cases_launch_every_decode_class_of_the_engine_at_its_smallest_and_largest_batch(built_lib, tmp_path):
+    """Every (cluster size, n_heads, n_kv) decode class the engine's plans launch (tp = 1 at TINY, MID, 8B and 70B shapes;
+    8B and 70B at tp 2, 4 and 8; decode batches 1..128), at the smallest and at the largest batch it is launched at, is
+    launched by a case of tests/test_decode_attention_sm90_gpu.py."""
+    spec = tmp_path / "decode_cases.json"
+    spec.write_text(json.dumps({"decode": [list(c) for c in DA.DECODE_CASES]}))
+    tested = run_logged(tmp_path, "decode_cases", [os.path.join(HERE, "support", "kernel_case_sweep.py"), str(spec)], parse=decode_launches)
+    assert tested == {(DA.cluster_size(sp), nh, nkv, B) for sp, nh, nkv, B in DA.DECODE_CASES}
+    engine = {}
+    for model, tp in DECODE_PLANS:
+        for c, nh, nkv, nb in _engine_plan(tmp_path, model, tp, DA.MAX_BATCH, parse=decode_launches):
+            engine.setdefault((c, nh, nkv), set()).add(nb)
+    assert {k[1:] for k in engine} == set(DA.HEADS_TP1 + DA.HEADS_SHARDS), sorted(engine)
+    assert {k[0] for k in engine} == {1, 2, 4, 8, 16} and max(max(b) for b in engine.values()) == DA.MAX_BATCH
+    missing = sorted(k + (nb,) for k, batches in engine.items() for nb in (min(batches), max(batches)) if k + (nb,) not in tested)
+    assert not missing, "the engine launches decode attention (cluster, n_heads, n_kv, batch) no GPU case runs: %s" % missing
+
+
+def test_decode_layer_chain_launches_what_the_engine_launches(built_lib, tmp_path):
+    """The decode layer chain of tests/test_gemv_sm90_gpu.py, layers 0 and 1 at B = 1..4, against the first two layers of
+    the engine's decode step at Llama-3-8B, tp = 1: the same kernels with the same grid, block, dynamic shared memory,
+    cluster, PDL flag and logged arguments, in the same order."""
+    spec = tmp_path / "chain.json"
+    spec.write_text(json.dumps({"chain": list(GV.CHAIN_BATCHES)}))
+    chain = run_logged(tmp_path, "chain", [os.path.join(HERE, "support", "kernel_case_sweep.py"), str(spec)], parse=launch_lines)
+    plan = _engine_plan(tmp_path, "8b", 1, 4, parse=launch_lines)
+    assert (GV.CHAIN_H, GV.CHAIN_QKV, GV.CHAIN_FFN) == (4096, 6144, 14336) and (GV.CHAIN_HEADS, GV.CHAIN_KV) == (32, 8)
+    for B in GV.CHAIN_BATCHES:
+        ours = chain["chain B=%d" % B]
+        steps = plan["decode B=%d" % B]
+        i = next(j for j, p in enumerate(steps) if short_name(p[0]) in DECODE_KERNELS and int(p[14]) == B)
+        engine = steps[i - 1: i + 9]
+        assert len(ours) == 10 and [short_name(p[0]) for p in engine[:2]] == ["gemv_ks_kernel", short_name(ours[1][0])], engine
+        assert short_name(engine[6][0]) in DECODE_KERNELS and (engine[1][11], engine[6][11]) == ("0", "1")   # layer 1: PDL
+        assert ours == engine, "B = %d: the chain launches\n%s\nthe engine\n%s" % (B, "\n".join(map(" ".join, ours)), "\n".join(map(" ".join, engine)))
+
+
+# teeth: the decode checkers of the GPU test applied on the CPU to a model of the kernels, right or wrong in one way
+DNH, DNKV, DLENS = 16, 2, (1, 33, 64, 65, 300)      # GQA group 8: two head groups of 4 share a kv head
+
+
+def _rotate(qkv, pos, table, nh, nkv, pos_shift=0, sin_sign=1.0, interleaved=False):
+    """rope_append's rotation of the q and k heads of the bf16 rows at pos in fp32, or wrong in one way: a rotated copy."""
+    B, nr = qkv.shape[0], nh + nkv
+    x = qkv[:, : nr * 128].reshape(B, nr, 128).float()
+    cs = table[pos.long() + pos_shift]
+    c, s = cs[:, None, :, 0], sin_sign * cs[:, None, :, 1]
+    a, b = (x[..., 0::2], x[..., 1::2]) if interleaved else (x[..., :64], x[..., 64:])
+    ra, rb = (a * c - b * s).to(torch.bfloat16), (b * c + a * s).to(torch.bfloat16)
+    rot = torch.stack([ra, rb], -1).flatten(-2) if interleaved else torch.cat([ra, rb], -1)
+    out = qkv.clone()
+    out[:, : nr * 128] = rot.reshape(B, nr * 128)
+    return out
+
+
+def _decode_case():
+    """A CPU pool with random context for DLENS and the qkv rows of this step and of the previous layer."""
+    pool = DA.Pool(DNKV, DLENS, 21, device="cpu")
+    gen = torch.Generator().manual_seed(22)
+    ctx_k = [torch.randn(n - 1, DNKV, 128, generator=gen).to(torch.bfloat16) for n in DLENS]
+    ctx_v = [torch.randn(n - 1, DNKV, 128, generator=gen).to(torch.bfloat16) for n in DLENS]
+    for i, n in enumerate(DLENS):
+        pool.write(i, 0, ctx_k[i], ctx_v[i])
+    qkv, prev = DA.qkv_rows(len(DLENS), DNH, DNKV, gen), DA.qkv_rows(len(DLENS), DNH, DNKV, gen, row0=1)
+    return pool, ctx_k, ctx_v, qkv, prev, torch.tensor(DLENS, dtype=torch.int32)
+
+
+def _decode_model(pool, qkv, seq_lens, table, stale_new=False, slot_shift=0, kv_shift=0, group4=False, **rot):
+    """A decode launch in fp64 on the CPU: (out, K pool, V pool).  Right, or wrong in one way: the rotation (_rotate's
+    knobs), the new token read from the stale page row, k appended slot_shift slots on or kv_shift kv heads over, q head h
+    reading kv head (h // 4) % n_kv (the head group's index instead of its kv head)."""
+    nh, nkv, g = DNH, DNKV, DNH // DNKV
+    r = _rotate(qkv, seq_lens - 1, table, nh, nkv, **rot)
+    kp, vp = pool.kp.clone(), pool.vp.clone()
+    outs = []
+    for b, L in enumerate(seq_lens.tolist()):
+        pos, row = L - 1, pool.bt[int(pool.rows[b])].long()
+        kn, vn = r[b, nh * 128:(nh + nkv) * 128].view(nkv, 128), qkv[b, (nh + nkv) * 128:].view(nkv, 128)
+        p_at = pos + slot_shift
+        kp[row[p_at // 64], (torch.arange(nkv) + kv_shift) % nkv, p_at % 64] = kn
+        vp[row[pos // 64], :, pos % 64] = vn
+        t = torch.arange(L)
+        k, v = pool.kp[row[t // 64], :, t % 64].clone(), pool.vp[row[t // 64], :, t % 64].clone()
+        if not stale_new:
+            k[pos], v[pos] = kn, vn
+        kv_of = (torch.arange(nh) // 4) % nkv if group4 else torch.arange(nh) // g
+        q = r[b, : nh * 128].view(nh, 128).double()
+        sc = torch.einsum("hd,shd->hs", q, k.double()[:, kv_of]) / 128 ** 0.5
+        outs.append(torch.einsum("hs,shd->hd", torch.softmax(sc, -1), v.double()[:, kv_of]).to(torch.bfloat16).flatten())
+    return torch.stack(outs), kp, vp
+
+
+def _decode_rejects(prev_rows=False, table=None, **knobs):
+    """(output elements over the bound, K pool words wrong, V pool words wrong) of the model, by the GPU test's checker."""
+    pool, ctx_k, ctx_v, qkv, prev, seq_lens = _decode_case()
+    real = _rope_table()
+    out, kp, vp = _decode_model(pool, prev if prev_rows else qkv, seq_lens, real if table is None else table, **knobs)
+    rot = _rotate(qkv, seq_lens - 1, real, DNH, DNKV)            # what rope_append computes for this step's rows
+    return DA.decode_rejects(out, kp, vp, pool.kp, pool.vp, pool.bt, pool.rows, seq_lens, qkv, rot, ctx_k, ctx_v, DNH, DNKV, 0.0)[:3]
+
+
+def test_decode_checkers_accept_a_correct_kernel():
+    assert _decode_rejects() == (0, 0, 0)
+
+
+def test_decode_checkers_reject_a_wrong_rotation():
+    identity = torch.zeros_like(_rope_table())
+    identity[..., 0] = 1
+    for knobs in (dict(table=identity), dict(pos_shift=1), dict(sin_sign=-1.0), dict(interleaved=True)):
+        n_out, n_k, _ = _decode_rejects(**knobs)
+        assert n_out > 0 and n_k > 0, knobs
+
+
+def test_decode_checkers_reject_the_stale_page_row_a_misplaced_append_another_head_groups_kv_and_the_previous_rows():
+    assert _decode_rejects(stale_new=True)[0] > 0
+    assert _decode_rejects(slot_shift=1)[1] > 0
+    assert _decode_rejects(kv_shift=1)[1] > 0
+    assert _decode_rejects(group4=True)[0] > 0
+    n_out, n_k, n_v = _decode_rejects(prev_rows=True)
+    assert n_out > 0 and n_k > 0 and n_v > 0
 
 
 # ------------------------------------------------------------------------------------------------------------- sampler --
